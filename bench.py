@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — headline benchmark: assembly Mbp polished / second (BASELINE.json).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload NAME]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload NAME] [--dump-outputs DIR]
 
 One step = one pass of the polish hot path (classify -> CIGAR walk + pileup -> vote + compaction) over one
 synthetic workload (default: BASELINE configs[1], one 5 Mbp contig at 100x, multi-mapped 150 bp pairs).
@@ -16,6 +16,8 @@ With N > 1 (torchrun, one rank per GPU) the contigs of ONE config-5-shaped assem
 families that cross contigs) shard across the ranks with no collective on the data path: every rank polishes its
 shard, ghost records included (weak scaling); time = max over ranks.
 --impl reference times the reference's CPU path (the oracle; the Rust reference cannot be built here) on rank 0.
+--dump-outputs DIR writes what the last timed step returned (rank 0) as DIR/<name>.npy, float32 / float64, at most 64 MB:
+two builds run with the same arguments polish the same seeded input, so their dumps compare array for array.
 """
 import argparse
 import json
@@ -40,11 +42,28 @@ WORKLOADS = {
 METRIC = "assembly Mbp polished/sec"
 
 
-def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return json.load(open(p)).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+HBM_PEAK_GBS = 3350.0     # NVIDIA H100 SXM data sheet (HBM3, 700 W card): the roofline denominator, not a measured rate
+DUMP_LIMIT = 64 << 20     # bytes --dump-outputs may write
+
+
+def dump_outputs(out_dir, sequences, changed, zero_depth, total_depth, n_aln_used):
+    """The polished contigs and their statistics as .npy files.  Bases are stored as their byte values in float32; when
+    they would not fit beside the rest, a fixed seeded sample of positions (and the positions themselves) is written."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    bases = np.frombuffer(b"".join(sequences), dtype=np.uint8)
+    arrs = {"contig_lengths": np.array([len(s) for s in sequences], dtype=np.float64),
+            "changed": np.array(changed, dtype=np.float64), "zero_depth": np.array(zero_depth, dtype=np.float64),
+            "total_depth": np.array(total_depth, dtype=np.float64), "n_aln_used": np.array([n_aln_used], dtype=np.float64)}
+    room = (DUMP_LIMIT - sum(a.nbytes for a in arrs.values()) - (1 << 20)) // 4
+    if bases.size <= room:
+        arrs["bases"] = bases.astype(np.float32)
+    else:
+        idx = np.sort(np.random.default_rng(0).choice(bases.size, size=room // 3, replace=False))
+        arrs["bases_sample"] = bases[idx].astype(np.float32)
+        arrs["bases_sample_index"] = idx.astype(np.float64)
+    for name, a in arrs.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 class ClockSampler:
@@ -75,6 +94,7 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": []}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         sm, mx, reasons = [], None, set()
         for s in self.samples:
             f = [x.strip() for x in s.split(",")]
@@ -145,7 +165,7 @@ def run_reference(args, rank, world):
         syn = api.Synth(seed=2, n_contigs=n_c, contig_len=clen, depth=depth)
         fa, sams = syn.write(d)
         bp = syn.total_bp
-        vals, sha = [], None
+        vals, sha, r = [], None, None
         for i in range(args.warmup + args.steps):
             dt, r = oracle_polish(fa, sams)
             sha = hashlib.sha256(r["fasta"]).hexdigest()
@@ -153,6 +173,8 @@ def run_reference(args, rank, world):
                 vals.append((bp / 1e6 / dt, dt, r["secs"]))
     finally:
         shutil.rmtree(d, ignore_errors=True)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, r["fasta"].split(b"\n")[1::2], r["changed"], r["zero_depth"], r["total_depth"], r["used_total"])
     v = sum(x[0] for x in vals) / len(vals)
     ms = 1e3 * sum(x[1] for x in vals) / len(vals)
     what = "the whole workload" if same else ("one contig of the %d-GPU workload's %d" % (world, (25 * world) // 4) if world > 1 else "a slice of the workload")
@@ -176,6 +198,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--wire4", action="store_true", help="e2e with the 4-bit arrays on the wire instead of the 2-bit format")
     ap.add_argument("--no-t3", action="store_true", help="skip the SAM-text-on-disk -> FASTA measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
@@ -283,8 +306,9 @@ def main():
     stage = {}
     dev_ms = 0.0
     launches = 0
-    for _ in range(args.steps):
-        r = ctx.polish_resident(fetch=False)
+    for i in range(args.steps):
+        # the last step also copies its result to the host when it is dumped (after the events that time the step)
+        r = ctx.polish_resident(fetch=bool(args.dump_outputs) and i == args.steps - 1)
         dev_ms += r["timing"]["total_ms"]
         launches += r["timing"]["launches"]
         for k, v in r["timing"].items():
@@ -294,6 +318,8 @@ def main():
     wall_ms = (time.perf_counter() - t0) * 1e3
     out_len = r["out_len"]
     ms_step = dev_ms / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, r["sequences"], r["changed"], r["zero_depth"], r["total_depth"], r["n_aln_used"])
 
     # ---------------- e2e: host buffers through pp_polish ----------------
     # (inputs in pinned host arrays, the result into caller-owned pinned buffers; the last result is checked against the
@@ -303,7 +329,7 @@ def main():
         e = ctx.polish_packed(cview, hv, into=out_res)
     barrier()
     t0 = time.perf_counter()
-    e2e_steps = max(3, min(args.steps, 10))
+    e2e_steps = args.steps
     e2e_each = []
     for _ in range(e2e_steps):
         t1 = time.perf_counter()
@@ -317,6 +343,13 @@ def main():
     d2h_bytes = int(e["out_len"]) + 8 * (3 * n_c + 1)
     ctx.free_pinned_result(out_res[1])
     clocks = sampler.stop() if rank == 0 else None      # sampled over both timed regions (kernel path + e2e)
+    if rank == 0:
+        try:
+            q = subprocess.run(["nvidia-smi", "-i", str(local), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                               capture_output=True, text=True, timeout=30).stdout.strip()
+        except Exception:
+            q = None
+        clocks["device"] = q or torch.cuda.get_device_name(local)       # the card and its power limit belong with the numbers
     d2h_bytes = int(e["out_len"]) + 8 * (3 * n_c + 1)
 
     # ---------------- T3: the whole command, SAM/FASTA text on disk (page cache warm) -> polished FASTA bytes ----------------
@@ -407,16 +440,10 @@ def main():
     total_bp, h2d_total, d2h_total, aln_total = tot.tolist()   # the whole job: every rank's contigs
 
     if rank == 0:
-        hbm, how = peaks()
+        hbm = HBM_PEAK_GBS
         ab = algorithmic_bytes(arrs, G, out_len)
         sc_ms = stage["tile_ms"] / args.steps
         k_bytes = ab["alignment_side"] + G                 # what one k_tile launch must move: every alignment record, CIGAR op and read base, and the draft
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tp):
-            tj = json.load(open(tp))
-            traffic = tj.get(args.workload) if world == 1 else None
-            traffic_src = "static, from profiles/traffic.json (%s); not measured in this run" % tj.get("source", "ncu --set full capture")
         line = {
             "metric": METRIC, "value": total_bp / 1e6 / (ms_step_max / 1e3), "unit": "Mbp/s", "n_gpus": world,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step_max, "higher_is_better": True,
@@ -427,7 +454,7 @@ def main():
                        "parallelism": (f"one assembly, contigs sharded over {world} ranks by pp_shards_build_assigned (ghost records), no collective on the data path"
                                        if world > 1 else "1 GPU"),
                        "timing": "CUDA events on the library stream, max over ranks",
-                       "cache": "inputs (%.0f MB packed) larger than the 126 MB L2" % (h2d_bytes / 1e6)},
+                       "cache": "inputs (%.0f MB packed) larger than the 50 MB L2" % (h2d_bytes / 1e6)},
             "e2e": {"value": total_bp / 1e6 / (e2e_ms_max / 1e3), "unit": "Mbp/s", "ms_per_step": e2e_ms_max,
                     "h2d_bytes_per_step": int(h2d_total), "d2h_bytes_per_step": int(d2h_total), "api": "pp_polish (host SoA in, host bases out)",
                     "wire": ("2-bit read bases, cigar_off and read_id rebuilt on the device (pp_alignments_to_2bit once per batch, outside the timed region like the packing; %d B/step as 4-bit)" % h2d_bytes_4bit
@@ -437,7 +464,7 @@ def main():
                     "last_step_ms": {k: round(v, 3) for k, v in e["timing"].items() if k.endswith("_ms") and v}},   # h2d = upload + position binning
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "kernel": "k_tile<4>", "achieved": k_bytes / 1e9 / (sc_ms / 1e3), "peak": hbm,
-                         "unit": "GB/s", "frac": k_bytes / 1e9 / (sc_ms / 1e3) / hbm, "traffic": traffic, "traffic_source": traffic_src, "peak_source": how,
+                         "unit": "GB/s", "frac": k_bytes / 1e9 / (sc_ms / 1e3) / hbm, "peak_source": "H100 SXM data sheet, 3.35 TB/s HBM3",
                          "algorithmic_bytes_per_launch": k_bytes, "kernel_ms": sc_ms,
                          "whole_path": {"algorithmic_bytes": ab["total"], "ms": ms_step, "achieved": ab["total"] / 1e9 / (ms_step / 1e3),
                                         "frac": ab["total"] / 1e9 / (ms_step / 1e3) / hbm}},

@@ -3,13 +3,13 @@
  * The reference (rrwick/Polypolish v0.6.1) is a monolithic Rust binary with no plugin/FFI surface, so the
  * drop-in boundary is cut at the function seams of its hot path (SURVEY.md §8b); each entry point below
  * names the reference function(s) it replaces.  Everything text-shaped (SAM/FASTA) stays on the host side of
- * the boundary; everything from packed records to polished bytes runs as sm_100a kernels.
+ * the boundary; everything from packed records to polished bytes runs as sm_90a kernels.
  *
  * Conventions: plain pointers and sizes, no C++/torch types; the caller owns every host buffer; the library
  * owns all device memory and streams inside pp_ctx; integer return codes (0 = ok, <0 = error) and
  * pp_last_error() for the message; no exceptions or exit() cross the boundary.  A pp_ctx is single-threaded
  * (the reference is single-threaded); multi-GPU = one ctx per GPU, one host thread (or process) each.
- * There is no CPU fallback: every compute entry point fails with PP_ERR_CUDA when no sm_100 device is usable.
+ * There is no CPU fallback: every compute entry point fails with PP_ERR_CUDA when no sm_90 (H100) device is usable.
  */
 #ifndef PP_ABI_H
 #define PP_ABI_H
@@ -321,8 +321,8 @@ int pp_get_parser(const pp_ctx* ctx);
 int pp_tok_set_readers(pp_ctx* ctx, int n);
 /* Optional (default 0): pp_tok_add_file(s) / pp_tok_prefetch stage the text with QUAL (column 11: 45 % of a bwa-mem line,
  * never read by polish, alignment.rs:49-98) replaced by "*", so that 40 % less crosses PCIe.  Same arrays, same result; it pays
- * only where the PCIe link is narrower than what the reader threads can strip (measured on this pod: 20-30 ms instead of
- * 13-20 ms per 626 MB file, i.e. slower).  `filter`, which reproduces its input lines, always uploads byte for byte.  With it on,
+ * only where the PCIe link is narrower than what the reader threads can strip (bench.py reports both as t3.ms and
+ * t3.strip_qual_ms).  `filter`, which reproduces its input lines, always uploads byte for byte.  With it on,
  * the line count in pp_tok_stats includes one comment line per upload slice. */
 int pp_tok_set_strip_qual(pp_ctx* ctx, int on);
 /* The resident dataset read back (tests: equality with the host packer's arrays).  pp_dataset_sizes fills the counts of

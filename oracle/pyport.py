@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY (imported by tests/test_golden.py and tests/test_pyport.py): it exists so that the golden
 fixtures and the C++ oracle are pinned by TWO separate readings of the Rust source instead of one.  It was written from
-/root/reference/src/*.rs directly (not from oracle/polypolish_oracle.cpp) and follows the reference's own structure:
+reference src/*.rs directly (not from oracle/polypolish_oracle.cpp) and follows the reference's own structure:
 strings, a dict per position, sequential float depth.  Pure-Python loops: small inputs only.
 
   alignment.rs:49-98    Alignment.new            alignment.rs:102-128  Alignment.new_quick

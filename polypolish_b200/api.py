@@ -97,7 +97,7 @@ def lib():
     p = lib_path()
     if not os.path.exists(p):
         raise PolypolishError(PP_ERR_CUDA, f"{p} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                                           "(nvcc, sm_100a). There is no CPU fallback.")
+                                           "(nvcc, sm_90a). There is no CPU fallback.")
     L = C.CDLL(p)
     L.pp_version.restype = C.c_char_p
     L.pp_last_error.restype = C.c_char_p
@@ -276,7 +276,7 @@ class Context:
         h = C.c_void_p()
         rc = L.pp_create(device, C.byref(h))
         if rc != PP_OK:
-            raise PolypolishError(rc, "pp_create failed: no usable sm_100 CUDA device (there is no CPU fallback)")
+            raise PolypolishError(rc, "pp_create failed: no usable sm_90 (H100) CUDA device (there is no CPU fallback)")
         self.h = h
 
     def _err(self, rc):

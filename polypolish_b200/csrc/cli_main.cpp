@@ -58,7 +58,7 @@ static void help_filter() {               // main.rs:46-75
     puts("      --high <HIGH>                High percentile threshold [default: 99.9]");
     puts("  -h, --help                       Print help");
     puts("  -V, --version                    Print version");
-    puts("\nB200 build, additive options: --device <N> (GPU, default 0), --quiet, --host-parse");
+    puts("\nH100 build, additive options: --device <N> (GPU, default 0), --quiet, --host-parse");
 }
 
 static void help_polish() {               // main.rs:77-108
@@ -84,7 +84,7 @@ static void help_polish() {               // main.rs:77-108
     puts("          Print help");
     puts("  -V, --version");
     puts("          Print version");
-    puts("\nB200 build, additive options: --device <N> (first GPU, default 0), --gpus <N> (contigs shard over N GPUs), --quiet, --host-parse");
+    puts("\nH100 build, additive options: --device <N> (first GPU, default 0), --gpus <N> (contigs shard over N GPUs), --quiet, --host-parse");
 }
 
 // clap accepts `--name=value`, `-m5` / `-m=5` and a `--` separator (everything after it is positional): normalise those forms
@@ -192,14 +192,14 @@ int main(int argc, char** argv) {
         const int base = restrict_visible_devices(device, gpus) ? 0 : device;
         std::vector<pp_ctx*> ctxs(gpus, nullptr);
         for (int g = 0; g < gpus; ++g)
-            if (pp_create(base + g, &ctxs[g]) != PP_OK) quit_with_error("no usable Blackwell (sm_100) GPU: this build has no CPU fallback");
+            if (pp_create(base + g, &ctxs[g]) != PP_OK) quit_with_error("no usable H100 (sm_90) GPU: this build has no CPU fallback");
         mark("contexts created");
         if (host_parse) pp_set_parser(ctxs[0], 1);
         std::vector<const char*> sams;
         for (size_t i = 1; i < pos.size(); ++i) sams.push_back(pos[i].c_str());
         char* out = nullptr;
         uint64_t n = 0;
-        if (!quiet) fprintf(stderr, "Starting Polypolish polish (B200 build %s, %d GPU%s)\n\n", pp_version(), gpus, gpus > 1 ? "s" : "");
+        if (!quiet) fprintf(stderr, "Starting Polypolish polish (H100 build %s, %d GPU%s)\n\n", pp_version(), gpus, gpus > 1 ? "s" : "");
         int rc = pp_polish_files_multi(ctxs.data(), gpus, pos[0].c_str(), sams.data(), (int)sams.size(), &prm, debug.empty() ? nullptr : debug.c_str(), &out, &n, quiet ? 0 : 1);
         if (rc != PP_OK) { std::string m = pp_last_error(ctxs[0]); for (auto c : ctxs) pp_destroy(c); quit_with_error(m); }
         mark("polished");
@@ -207,7 +207,7 @@ int main(int argc, char** argv) {
         if (!quiet) fprintf(stderr, "Finished!\n");
         mark("output written");
         // A one-shot process has nothing left to do: the contexts, the driver's tear-down and the runtime's static destructors
-        // (30 - 1000 ms on these boxes) are skipped - the kernel reclaims everything.  Output files first.
+        // (up to a second) are skipped - the kernel reclaims everything.  Output files first.
         if (fflush(stdout) != 0 || ferror(stdout)) quit_with_error("unable to write to stdout");
         fflush(stderr);
         _exit(0);
@@ -237,9 +237,9 @@ int main(int argc, char** argv) {
             usage_error("the following required arguments were not provided:\n  --in1 <IN1>\n  --in2 <IN2>\n  --out1 <OUT1>\n  --out2 <OUT2>");
         const int base = restrict_visible_devices(device, 1) ? 0 : device;
         pp_ctx* ctx = nullptr;
-        if (pp_create(base, &ctx) != PP_OK) quit_with_error("no usable Blackwell (sm_100) GPU: this build has no CPU fallback");
+        if (pp_create(base, &ctx) != PP_OK) quit_with_error("no usable H100 (sm_90) GPU: this build has no CPU fallback");
         if (host_parse) pp_set_parser(ctx, 1);
-        if (!quiet) fprintf(stderr, "Starting Polypolish filter (B200 build %s)\n\n", pp_version());
+        if (!quiet) fprintf(stderr, "Starting Polypolish filter (H100 build %s)\n\n", pp_version());
         int rc = pp_filter_files(ctx, in1.c_str(), in2.c_str(), out1.c_str(), out2.c_str(), orientation.c_str(), low, high, quiet ? 0 : 1);
         if (rc != PP_OK) { std::string m = pp_last_error(ctx); pp_destroy(ctx); quit_with_error(m); }
         if (!quiet) fprintf(stderr, "Finished!\n");
@@ -257,7 +257,7 @@ int main(int argc, char** argv) {
             const std::string& a = tok[i].text;
             if (tok[i].positional) { pos.push_back(a); continue; }
             if (a == "-h" || a == "--help") {
-                puts("filter paired-end alignments based on insert size, then polish the assembly with the filtered alignments (one pass, B200 build only)\n");
+                puts("filter paired-end alignments based on insert size, then polish the assembly with the filtered alignments (one pass, H100 build only)\n");
                 puts("Usage: polypolish filter-polish [OPTIONS] --in1 <IN1> --in2 <IN2> <ASSEMBLY>\n");
                 puts("Options: those of `filter` (--out1 / --out2 optional: written only when given) and of `polish` (except --debug)");
                 return 0;
@@ -284,9 +284,9 @@ int main(int argc, char** argv) {
             usage_error("the following required arguments were not provided:\n  --in1 <IN1>\n  --in2 <IN2>\n  <ASSEMBLY>");
         const int base = restrict_visible_devices(device, 1) ? 0 : device;
         pp_ctx* ctx = nullptr;
-        if (pp_create(base, &ctx) != PP_OK) quit_with_error("no usable Blackwell (sm_100) GPU: this build has no CPU fallback");
+        if (pp_create(base, &ctx) != PP_OK) quit_with_error("no usable H100 (sm_90) GPU: this build has no CPU fallback");
         if (host_parse) pp_set_parser(ctx, 1);
-        if (!quiet) fprintf(stderr, "Starting Polypolish filter + polish (B200 build %s)\n\n", pp_version());
+        if (!quiet) fprintf(stderr, "Starting Polypolish filter + polish (H100 build %s)\n\n", pp_version());
         char* out = nullptr;
         uint64_t n = 0;
         int rc = pp_filter_polish_files(ctx, pos[0].c_str(), in1.c_str(), in2.c_str(), out1.empty() ? nullptr : out1.c_str(), out2.empty() ? nullptr : out2.c_str(),

@@ -1,6 +1,6 @@
 // fasta.cpp — host-side FASTA loader and small text utilities.
 //
-// Behavioural mirror of misc::load_fasta (/root/reference/src/misc.rs:38-167): gzip detected by the
+// Behavioural mirror of misc::load_fasta (reference src/misc.rs:38-167): gzip detected by the
 // magic bytes 1f 8b (:81-99), lines split like Rust's lines(), blank lines skipped (:111), header =
 // name up to the first Unicode whitespace + description (:118-120), sequence lines concatenated and
 // ASCII-upper-cased (:114,129), then the checks of check_load_fasta (:56-75) with the same messages.

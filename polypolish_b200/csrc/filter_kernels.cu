@@ -1,6 +1,6 @@
 // filter_kernels.cu — `polypolish filter` on the device: insert-size thresholds + per-alignment pair QC.
 //
-// Replaces (reference = /root/reference/src/filter.rs):
+// Replaces (reference = Polypolish src/filter.rs):
 //   load_alignments' name-keyed grouping     :91-145   -> k_f_build   (per-name counts + linked lists)
 //   get_insert_size_thresholds               :148-186  -> k_f_pairs   (unique pairs: orientation, insert size)
 //   get_orientation / get_insert_size        :189-218  -> orient_insert()
@@ -21,6 +21,7 @@
 
 // context pieces shared with polish_kernels.cu
 int pp_ctx_device(pp_ctx* ctx);
+int pp_ctx_sm_count(pp_ctx* ctx);
 cudaStream_t pp_ctx_stream(pp_ctx* ctx);
 int pp_ctx_fail_cuda(pp_ctx* ctx, cudaError_t e, const char* what, const char* file, int line);
 void* pp_ctx_scratch(pp_ctx* ctx, size_t bytes);       // grows a ctx-owned device buffer; nullptr on failure
@@ -201,7 +202,7 @@ int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, p
     CKF(cudaMemsetAsync(base + zero_end, 0xFF, ff_end - zero_end, s));
     CKF(cudaEventRecord(pp_ctx_event(ctx, 1), s));
 
-    auto grid = [&](size_t n) { return (unsigned)std::min<size_t>(std::max<size_t>((n + 255) / 256, 1), 148 * 8); };
+    auto grid = [&](size_t n) { return (unsigned)std::min<size_t>(std::max<size_t>((n + 255) / 256, 1), (size_t)pp_ctx_sm_count(ctx) * 8); };
     uint32_t launches = 0;
     for (int k = 0; k < 2; ++k)
         if (in[k].n) { k_f_build<<<grid(in[k].n), 256, 0, s>>>(f, k); launches++; }

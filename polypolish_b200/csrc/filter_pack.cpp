@@ -1,6 +1,6 @@
 // filter_pack.cpp — host text side of `polypolish filter`: SAM text -> per-mate record arrays, and the SAM writer.
 //
-// Restates the TEXT handling of /root/reference/src/filter.rs only:
+// Restates the TEXT handling of reference src/filter.rs only:
 //   load_alignments_one_file :110-145 with Alignment::new_quick (alignment.rs:102-128): every non-'@' line is parsed
 //       (an empty line is "too few columns"), unaligned records are skipped, aligned ones are keyed by QNAME + mate;
 //   Alignment::get_ref_end (alignment.rs:138-149) for the read-end coordinate;

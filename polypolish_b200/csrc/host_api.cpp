@@ -1,8 +1,8 @@
 // host_api.cpp — whole-command drivers above the C-ABI compute calls.
 //
 // Mirrors the reference's command drivers (same option checks, same error text, same stdout bytes):
-//   polish::polish            /root/reference/src/polish.rs:26-38   (+ :93-134 loading, :137-203 output)
-//   filter::filter            /root/reference/src/filter.rs:26-37   (+ :273-349 SAM re-streaming)
+//   polish::polish            reference src/polish.rs:26-38   (+ :93-134 loading, :137-203 output)
+//   filter::filter            reference src/filter.rs:26-37   (+ :273-349 SAM re-streaming)
 // Text (FASTA/SAM) is handled here on the host; all per-alignment / per-position work is behind
 // pp_polish() / pp_filter() on the device.  There is no CPU fallback for that work.
 #include <chrono>

@@ -1,7 +1,7 @@
-// polish_dev.cuh — the polish hot path as sm_100a device code.  Included by polish_kernels.cu (nvcc; host side, C ABI) and,
+// polish_dev.cuh — the polish hot path as sm_90a device code.  Included by polish_kernels.cu (nvcc; host side, C ABI) and,
 // for logic checks without a GPU, by tests/emu/emu_polish.cpp (g++ with tests/emu/cuda_emu.h standing in for CUDA).
 //
-// Replaces, on the device (reference = /root/reference/src):
+// Replaces, on the device (reference = Polypolish v0.6.1, src/):
 //   process_one_read            alignment.rs:275-305  -> k_goodk (goodness, k = #good per read group, --careful, unknown-contig /
 //                                                         CIGAR errors), per call, SAM order
 //   get_read_bases_for_each_target_base + trim_bases_for_homopolymers
@@ -426,7 +426,7 @@ __global__ void __launch_bounds__(256) k_tile_weight(DevData d, uint32_t* __rest
 // GLOBALK = false: k of a multi-record group is counted right here (its records are consecutive alignments);
 // GLOBALK = true: k comes from k_classify_multi (fallback for huge groups).
 // ------------------------------------------------------------------------------------------------------
-// (four alignments per thread with 16-byte loads were measured: 0.054 ms against 0.044 ms for this one-per-thread form)
+// (four alignments per thread with 16-byte loads were measured slower than this one-per-thread form)
 struct PrepShared {
     uint32_t rid[PR_THREADS];
     uint8_t good[PR_THREADS];
@@ -1009,7 +1009,7 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, u
 
 // Everything that is not the plain fast walk (queued reads, the long list, a queue that overflowed): the two-segment fast walk for
 // one-indel reads, else the general walk.  (Inlined on purpose: as an out-of-line function - half the code size - the calls cost
-// the hot loop its registers, k_tile 0.53 -> 0.75 ms.)
+// the hot loop its registers and k_tile was measured markedly slower.)
 template <int BITS>
 __device__ __forceinline__ uint32_t slow_walk(const DevData* d, TileShared* sh, uint32_t P0, TileRec r, uint32_t slot, uint32_t k) {
     TileCtx<BITS> S{*d, *sh, P0};
@@ -1239,7 +1239,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         // The slots of the tile's bins and of the `lb` bins before it - one contiguous range of the binned dataset - and the first two
         // chunks' records: a chain of four dependent trips to memory (bin bounds, record, its k word, ...) that now runs under phase A.
         // (taking the next tile's ticket a tile early, to hide these trips, was measured: the greedy heaviest-first schedule then
-        // looks one tile ahead and the kernel's tail grows - 0.504 -> 0.548 ms)
+        // looks one tile ahead and the kernel's tail grows)
         const uint32_t b0 = P0 >> PP_BIN_SHIFT;
         const uint32_t lo = d.bin_start[b0 >= lb ? b0 - lb : 0u];
         const uint32_t hi = d.bin_start[min(b0 + (uint32_t)(TL_T / PP_BIN), d.n_bins)];
@@ -1510,8 +1510,10 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
 static_assert(TL_PER_THREAD == 4, "the verdict store packs four positions per thread");
 
 #if !defined(PP_EMULATE)
+// One CTA per SM: built for sm_90a, the body needs ~100 registers per thread.  Capped at 64 for two CTAs per SM it spills, and on an
+// H100 (400 W) the tile kernel took 0.79 ms per 5 Mbp x 100x call that way against 0.71 ms with one CTA per SM.
 template <int BITS>
-__global__ void __launch_bounds__(TL_THREADS, 2) k_tile(DevData d, VoteParams vp) {
+__global__ void __launch_bounds__(TL_THREADS, 1) k_tile(DevData d, VoteParams vp) {
     extern __shared__ __align__(16) unsigned char tile_smem[];
     tile_body<BITS>(d, vp, *reinterpret_cast<TileShared*>(tile_smem));
 }

@@ -50,7 +50,7 @@ extern "C" int pp_create(int device, pp_ctx** out) {
     ctx->device = device;
     if (cudaSetDevice(device) != cudaSuccess) { delete ctx; return PP_ERR_CUDA; }
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10) { delete ctx; return PP_ERR_CUDA; }
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) { delete ctx; return PP_ERR_CUDA; }   // sm_90a code loads on compute capability 9.0 only
     ctx->sm_count = prop.multiProcessorCount;
     if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return PP_ERR_CUDA; }
     if (cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return PP_ERR_CUDA; }
@@ -89,6 +89,7 @@ extern "C" const char* pp_last_error(const pp_ctx* ctx) { return ctx ? ctx->err.
 // internal (host_api.cpp, filter_kernels.cu): shared access to the context
 int pp_ctx_fail(pp_ctx* ctx, int code, const char* msg) { ctx->err = msg; return code; }
 int pp_ctx_device(pp_ctx* ctx) { return ctx->device; }
+int pp_ctx_sm_count(pp_ctx* ctx) { return ctx->sm_count; }
 cudaStream_t pp_ctx_stream(pp_ctx* ctx) { return ctx->stream; }
 cudaEvent_t pp_ctx_event(pp_ctx* ctx, int i) { return ctx->ev[i]; }
 void pp_ctx_count_launches(pp_ctx* ctx, uint32_t n) { ctx->launches = n; }

@@ -48,7 +48,7 @@ struct pp_ctx {
     // dataset facts
     uint64_t n_aln = 0, n_reads = 0, n_ops = 0, seq_bytes = 0, G = 0;
     uint32_t n_contigs = 0, seq_bits = 4;
-    int sm_count = 148;
+    int sm_count = 132;
     uint32_t launches = 0;
     // sizes that adapt when a call overflows them (kept across calls on the same dataset)
     uint32_t node_cap = 0;

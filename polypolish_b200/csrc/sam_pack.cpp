@@ -1,8 +1,8 @@
 // sam_pack.cpp — SAM text -> packed struct-of-arrays alignments (pp_alignments) for the polish path.
 //
 // Host side of the boundary: restates the TEXT handling of the reference, nothing else.
-//   add_to_pileup   /root/reference/src/alignment.rs:225-272  (line loop, '@'/empty skipping, grouping)
-//   Alignment::new  /root/reference/src/alignment.rs:49-98    (columns, FLAG/POS, NM / ZP tags, CIGAR check)
+//   add_to_pileup   reference src/alignment.rs:225-272  (line loop, '@'/empty skipping, grouping)
+//   Alignment::new  reference src/alignment.rs:49-98    (columns, FLAG/POS, NM / ZP tags, CIGAR check)
 //   get_expanded_cigar :325-346 (validation only: the CIGAR is kept run-length encoded, never expanded)
 //   get_read_seq_from_alignments :311-322 and add_read_seq :161-167 (source sequence of SEQ="*" records)
 // Everything downstream (goodness, k, CIGAR walk, trim, pileup, vote) happens on the device.

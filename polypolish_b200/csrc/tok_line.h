@@ -4,10 +4,10 @@
 // code is exercised on the CPU by tests/tok_harness.cpp against the host packer (sam_pack.cpp), which stays the
 // normative text layer: whatever this code is not sure about is answered with LK_HOST and the host packer decides
 // (result or the reference's error text).  What is restated here:
-//   Alignment::new          /root/reference/src/alignment.rs:49-98   columns, FLAG/POS, NM / ZP tags
-//   get_expanded_cigar      /root/reference/src/alignment.rs:325-346 validation (\d+[MIDNSHP=X] tokens or "*")
-//   add_to_pileup           /root/reference/src/alignment.rs:238-263 '@'/empty skipping, unaligned skipping, grouping rule
-//   process_one_read        /root/reference/src/alignment.rs:275-295 source sequence of SEQ="*" records
+//   Alignment::new          reference src/alignment.rs:49-98   columns, FLAG/POS, NM / ZP tags
+//   get_expanded_cigar      reference src/alignment.rs:325-346 validation (\d+[MIDNSHP=X] tokens or "*")
+//   add_to_pileup           reference src/alignment.rs:238-263 '@'/empty skipping, unaligned skipping, grouping rule
+//   process_one_read        reference src/alignment.rs:275-295 source sequence of SEQ="*" records
 #pragma once
 #include <stdint.h>
 #include <string.h>
@@ -42,7 +42,7 @@ struct Txt {
         return (uint8_t)(w >> (8 * (p & 7)));
     }
     // Position of the first '\t' in [p, e), or e.  (Word-at-a-time searches - a 64-bit zero-byte test, per-byte SIMD compares on
-    // the two halves - were measured slower on the device than this loop over the cached word: 1.68 / 2.6 ms against 1.50 ms.)
+    // the two halves - were measured slower on the device than this loop over the cached word.)
     TK_HD uint64_t find_tab(uint64_t p, uint64_t e) {
         while (p < e && at(p) != '\t') ++p;
         return p;

@@ -1,6 +1,6 @@
 """Second restatement as cross-check: oracle/pyport.py (plain Python, written from the Rust source independently of the C++
 oracle) against the golden fixtures and against the C++ oracle on fuzz cases.  Two separate readings of
-/root/reference/src/*.rs have to agree byte for byte on FASTA, debug TSV, statistics and filtered SAM."""
+reference src/*.rs have to agree byte for byte on FASTA, debug TSV, statistics and filtered SAM."""
 import importlib.util
 import json
 import os

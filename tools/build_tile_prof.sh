@@ -5,10 +5,10 @@
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p build_ab/prof
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wno-unused-function,-ffp-contract=off -fmad=false -DPP_TILE_PROF"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wno-unused-function,-ffp-contract=off -fmad=false -DPP_TILE_PROF"
 for f in polish_kernels.cu filter_kernels.cu tok_kernels.cu fasta.cpp sam_pack.cpp filter_pack.cpp host_api.cpp synth.cpp shard.cpp; do
   nvcc $FLAGS -x cu -c polypolish_b200/csrc/$f -o build_ab/prof/${f%.*}.o &
 done
 wait
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o build_ab/libpp_prof.so build_ab/prof/*.o -lz -lpthread
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o build_ab/libpp_prof.so build_ab/prof/*.o -lz -lpthread
 echo build_ab/libpp_prof.so
