@@ -21,9 +21,12 @@
 //     (~0.3 % of bases); count[draft base] = cover - sum(everything explicit); 32-bit counters (pileup.rs:33-37);
 //   * alleles other than A,C,G,T,"-" (N / IUPAC bases, insertions): one node per distinct (position, allele) in a
 //     per-position chain with an exact count (the reference's HashMap<String,u32>, pileup.rs:40,62);
-//   * depth: where every covering alignment has k == 1 the f64 depth equals cover exactly; 128-position sub-tiles that see an
-//     alignment with k != 1 get the reference's sequential f64 sum re-done in SAM order by one warp that merges the (already
-//     SAM-ordered) bins overlapping the sub-tile by alignment index (pileup.rs:64, alignment.rs:288);
+//   * depth: where every covering alignment has k == 1 the f64 depth equals cover exactly.  Alignments with k != 1 also add
+//     2^40 - round(2^40 / k) to a 64-bit fixed-point "deficit" (interval add + prefix sum like cover), so cover - deficit * 2^-40
+//     is the depth to within a proven bound (depth_bounds).  The vote only needs depth through four monotone tests; where both
+//     ends of the bound give the same answers the vote is the reference's.  Only a 128-position sub-tile with a position whose
+//     bound straddles a threshold gets the reference's sequential f64 sum re-done in SAM order, by one warp that merges the
+//     (already SAM-ordered) bins overlapping the sub-tile by alignment index (pileup.rs:64, alignment.rs:288);
 //   * the vote runs straight out of shared memory: the counters never exist in HBM, nothing has to be zeroed per call but
 //     4 B/bp of chain heads, and the working set per CTA does not depend on the assembly size (no L2 cliff).
 // Everything is integer / byte work bounded by HBM bandwidth: no tensor cores.
@@ -152,6 +155,32 @@ __constant__ uint8_t c_comp[256];      // misc.rs:170-182 complement_base on upp
 __constant__ char c_nib2asc[16] = {'=', 'A', 'C', 'M', 'G', 'R', 'S', 'V', 'T', 'W', 'Y', 'H', 'K', 'D', 'B', 'N'};
 #endif
 
+#if defined(PP_EMULATE)
+// Directed rounding on the CPU: the round-to-nearest result, stepped one ulp in the rounding direction when the exact result
+// (its error term from TwoSum / FMA) lies beyond it.
+static inline double emu_step(double r, double err, bool up) {
+    return (up ? err > 0.0 : err < 0.0) ? std::nextafter(r, up ? INFINITY : -INFINITY) : r;
+}
+static inline double emu_add(double a, double b, bool up) {
+    volatile double r = a + b;
+    const double bv = r - a, err = (a - (r - bv)) + (b - bv);
+    return emu_step(r, err, up);
+}
+static inline double __dadd_ru(double a, double b) { return emu_add(a, b, true); }
+static inline double __dsub_rd(double a, double b) { return emu_add(a, -b, false); }
+static inline double __dsub_ru(double a, double b) { return emu_add(a, -b, true); }
+static inline double __dmul_ru(double a, double b) { volatile double r = a * b; return emu_step(r, std::fma(a, b, -r), true); }
+static inline double emu_ull2double(unsigned long long x, bool up) {
+    const double r = (double)x;                               // round to nearest
+    const bool above = r >= 18446744073709551616.0 || (unsigned long long)r > x, below = r < 18446744073709551616.0 && (unsigned long long)r < x;
+    if (up ? below : above) return std::nextafter(r, up ? INFINITY : -INFINITY);
+    return r;
+}
+static inline double __ull2double_rd(unsigned long long x) { return emu_ull2double(x, false); }
+static inline double __ull2double_ru(unsigned long long x) { return emu_ull2double(x, true); }
+static inline double __ull2double_rn(unsigned long long x) { return (double)x; }
+#endif
+
 __device__ __forceinline__ uint32_t brev4(uint32_t c) {   // complement of a BAM nibble = 4-bit reversal
     return __brev(c) >> 28;
 }
@@ -251,6 +280,44 @@ __device__ __forceinline__ uint32_t bankers_rounding(double x) {
     if (fr < 0.5) return rd;
     if (fr > 0.5) return rd + 1;
     return rd + (rd & 1u);
+}
+
+// Everything the vote reads from depth (pileup.rs:70-72, 76): the valid and invalid thresholds and the low-depth test.  All three
+// are monotone non-decreasing in depth (IEEE multiplication by a non-negative constant and bankers_rounding both are).
+struct Thresholds { uint32_t vt, it; bool low; };
+__device__ __forceinline__ Thresholds vote_thresholds(const DevParams& prm, double depth) {
+    return Thresholds{max(prm.min_depth, bankers_rounding(__dmul_rn(depth, prm.fv))), bankers_rounding(__dmul_rn(depth, prm.fi)),
+                      depth < (double)prm.min_depth};
+}
+__device__ __forceinline__ bool same_thresholds(const DevParams& prm, double a, double b) {
+    const Thresholds x = vote_thresholds(prm, a), y = vote_thresholds(prm, b);
+    return x.vt == y.vt && x.it == y.it && x.low == y.low;
+}
+
+// The depth of a position from its cover (n covering alignments, an exact integer) and its fixed-point deficit M = sum over the
+// covering alignments with k != 1 of 2^40 - r_k, r_k = round(2^40 / k) (depth_deficit).  The reference's depth d_ref is the
+// sequential f64 sum, in SAM order, of fl(1/k) over the covering alignments; T = sum of 1/k is the exact value.
+//   * fixed point: |r_k 2^-40 - 1/k| <= 2^-41 and the k == 1 terms are exact, so d_fx = n - M 2^-40 has |d_fx - T| <= m 2^-41,
+//     m = covering alignments with k != 1 <= n;
+//   * the reference: fl(1/k) = (1/k)(1 + e), |e| <= u = 2^-53, then n - 1 additions of non-negative terms, so
+//     |d_ref - T| <= gamma_n T with gamma_n = n u / (1 - n u) (Higham, Accuracy and Stability, Lemma 3.1 and §4.2), and T <= n;
+//     for n u <= 1/2, gamma_n T <= 2 n^2 u = n^2 2^-52;
+//   * so |d_ref - d_fx| <= E = n 2^-41 + n^2 2^-52, and d_fx itself is bracketed by converting M to double rounded down and up
+//     (scaling by 2^-40 is exact).  Every step below rounds outwards, so [lo, hi] contains d_ref.
+// M < 2^63 (no wrap of the 64-bit prefix sum) needs m < 2^23: positions with n >= TL_DEF_COVER are not bounded here.
+#define TL_DEF_COVER (1u << 23)
+struct DepthBounds { double lo, hi, fx; };
+__device__ __forceinline__ DepthBounds depth_bounds(uint32_t cover, unsigned long long deficit) {
+    const double n = (double)cover;
+    const double e = __dadd_ru(n * 0x1p-41, __dmul_ru(n, n) * 0x1p-52);
+    DepthBounds b;
+    b.lo = __dsub_rd(__dsub_rd(n, __ull2double_ru(deficit) * 0x1p-40), e);
+    b.hi = __dadd_ru(__dsub_ru(n, __ull2double_rd(deficit) * 0x1p-40), e);
+    b.fx = __dsub_rn(n, __ull2double_rn(deficit) * 0x1p-40);
+    return b;
+}
+__device__ __forceinline__ unsigned long long depth_deficit(uint32_t k) {   // 2^40 - round(2^40 / k), k >= 2
+    return (1ull << 40) - ((1ull << 40) + k / 2) / k;
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -643,8 +710,8 @@ template <int BITS>
 __device__ __forceinline__ PosOut vote_position(const OthCtx& oc, const DevParams& prm, uint32_t pos, uint32_t orig, double depth,
                                                 uint32_t cA, uint32_t cC, uint32_t cG, uint32_t cT, uint32_t cDel,
                                                 uint32_t matched, uint32_t n_other, pp_debug_pos* dbg) {
-    const uint32_t vt = max(prm.min_depth, bankers_rounding(__dmul_rn(depth, prm.fv)));
-    const uint32_t it = bankers_rounding(__dmul_rn(depth, prm.fi));
+    const Thresholds th = vote_thresholds(prm, depth);
+    const uint32_t vt = th.vt, it = th.it;
     Tally t{0, 0, -1, 0};
     tally(t, cA, vt, it, 0, 0);
     tally(t, cC, vt, it, 1, 0);
@@ -657,7 +724,7 @@ __device__ __forceinline__ PosOut vote_position(const OthCtx& oc, const DevParam
     o.rec = 0;
     o.packed = (orig == '-' ? 0u : 1u) | (orig << 16);
     uint32_t status;                                          // 0 low_depth 1 none 2 multiple 3 too_close 4 kept 5 changed
-    if (depth < (double)prm.min_depth) status = 0;
+    if (th.low) status = 0;
     else if (t.nvalid == 0) status = 1;
     else if (t.nvalid > 1) status = 2;
     else if (t.ninter > 0) status = 3;
@@ -706,11 +773,14 @@ struct WalkStage {                                     // per warp: staging of t
 
 struct TileShared {
     int cdiff[TL_T + 4];                               // cover: +1 / -1 at interval ends, after the prefix sum = cover[p]
-    int mdiff[TL_T + 4];                               // the same restricted to alignments of reads with k != 1
     uint32_t ex[4][TL_T];                              // A, C, G, T entries that differ from the draft base
     uint32_t del[TL_T];                                // "-" entries
     uint32_t oth[TL_T];                                // entries carrying any other allele (their distinct strings: the global chains)
-    double depth[TL_T];                                // ordered f64 depth, valid in flagged sub-tiles
+    union {                                            // (per position both belong to the thread, then the warp, that votes on it)
+        unsigned long long deficit[TL_T + 4];          // fixed-point depth deficit of k != 1 alignments (depth_bounds): +d / -d at
+                                                       // interval ends, after the prefix sum the deficit of the position
+        double depth[TL_T];                            // ordered f64 depth, written over the deficit in sub-tiles that walk
+    };
     unsigned long long dn[TL_DN_WORDS + 2];            // 4-bit draft codes, 16 per word, position -32 first
     WalkStage wstage[TL_THREADS / 32];                 // ordered-depth merge staging, one per warp
     uint32_t queue[TL_QCAP];                           // sorted slots waiting for the two-segment / general walk
@@ -719,8 +789,9 @@ struct TileShared {
     unsigned long long s_total;
     long long s_delta[TL_THREADS / 32];
     uint32_t tile;
-    uint32_t subflags;                                 // sub-tiles that see k != 1 coverage
+    uint32_t any_multi;                                // an alignment with k != 1 touches the tile (the deficit is not all zero)
     double inv_k[TL_INV_K + 1];                        // 1.0 / k for small k (the ordered-depth walk divides once per slot otherwise)
+    unsigned long long def_k[TL_INV_K + 1];            // depth_deficit(k) for small k (add_interval divides otherwise)
 };
 
 template <int BITS> struct TileCtx {
@@ -752,13 +823,17 @@ template <int BITS> struct TileCtx {
         if (c >= 0) atomicAdd(&sh.ex[c][pos - P0], 1u);
         else push_other(pos, aln, ri, 1, 1ull | ((unsigned long long)s << (BITS == 4 ? 4 : 8)));
     }
-    // an alignment keeps entries [gstart, gstart + nkept): interval add restricted to the tile
-    __device__ __forceinline__ void add_interval(uint32_t gstart, uint32_t nkept, bool multi) {
+    // an alignment of a read with k good alignments keeps entries [gstart, gstart + nkept): interval add restricted to the tile
+    __device__ __forceinline__ void add_interval(uint32_t gstart, uint32_t nkept, uint32_t k) {
         const long long a64 = (long long)gstart - (long long)P0, b64 = a64 + (long long)nkept;
         const int a = (int)max(a64, 0ll), b = (int)min(b64, (long long)TL_T);
         if (b <= a) return;
         atomicAdd(&sh.cdiff[a], 1); atomicAdd(&sh.cdiff[b], -1);
-        if (multi) { atomicAdd(&sh.mdiff[a], 1); atomicAdd(&sh.mdiff[b], -1); }
+        if (k != 1) {
+            const unsigned long long dk = k <= (uint32_t)TL_INV_K ? sh.def_k[k] : depth_deficit(k);
+            atomicAdd(&sh.deficit[a], dk); atomicAdd(&sh.deficit[b], 0ull - dk);
+            sh.any_multi = 1u;
+        }
     }
     // 32 draft codes for tile-relative positions [rel0, rel0 + 32), rel0 in (-32, T)
     __device__ __forceinline__ void draft32(int rel0, unsigned long long& d0, unsigned long long& d1) const {
@@ -841,7 +916,7 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k)
     const unsigned long long nk64 = (E - run >= 1) ? (E - run - 1) : 0;
     if ((unsigned long long)gstart + nk64 > r.cend) { report_error(d.st, aln, ERR_OOB); return 0; }
     const uint32_t nkept = (uint32_t)nk64;
-    S.add_interval(gstart, nkept, k != 1);
+    S.add_interval(gstart, nkept, k);
     // positions of this tile the alignment can touch: entries [e_lo, e_hi)
     const long long off = (long long)S.P0 - (long long)gstart;
     const unsigned long long e_lo = off > 0 ? (unsigned long long)off : 0ull;
@@ -927,7 +1002,7 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, u
     const uint32_t E = one ? (is_del ? len + ib : len - ib) : len;
     const uint32_t nkept = E - run - 1;                         // run < 8 < entries of the last run
     if ((unsigned long long)r.gstart + nkept > r.cend) { report_error(S.d.st, aln, ERR_OOB); return 0; }
-    S.add_interval(r.gstart, nkept, k != 1);
+    S.add_interval(r.gstart, nkept, k);
     const long long g0 = (long long)r.gstart - (long long)S.P0;
     if (g0 >= (long long)TL_T || g0 + (long long)nkept <= 0) return nkept;
     const uint32_t* dn32 = reinterpret_cast<const uint32_t*>(S.sh.dn);
@@ -1223,10 +1298,13 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
     oc.nodes = d.nodes; oc.head = d.oth_head;
     oc.sr = SeqRef{d.seq_pool, d.seq_off, d.seq_len, d.flags};
 
-    if (tid <= (uint32_t)TL_INV_K) sh.inv_k[tid] = tid ? __ddiv_rn(1.0, (double)tid) : 0.0;   // the same correctly rounded quotients, made once
+    if (tid <= (uint32_t)TL_INV_K) {                                           // the same correctly rounded quotients, made once
+        sh.inv_k[tid] = tid ? __ddiv_rn(1.0, (double)tid) : 0.0;
+        sh.def_k[tid] = tid > 1 ? depth_deficit(tid) : 0ull;
+    }
     for (;;) {
         __syncthreads();                                                       // everyone is done with the previous tile
-        if (tid == 0) { sh.tile = atomicAdd(&d.st->ticket, 1u); sh.subflags = 0; sh.qn = 0; }
+        if (tid == 0) { sh.tile = atomicAdd(&d.st->ticket, 1u); sh.any_multi = 0; sh.qn = 0; }
         __syncthreads();
         if (sh.tile >= d.n_tiles) break;
         const uint32_t tile = d.tile_order[sh.tile];
@@ -1256,7 +1334,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         // ---- phase A: clear the counters, stage the draft as 4-bit codes
         {
             uint4* z = reinterpret_cast<uint4*>(sh.cdiff);
-            const uint32_t nz = (uint32_t)((size_t)((char*)sh.depth - (char*)sh.cdiff) / 16);   // cdiff, mdiff, ex, del, oth
+            const uint32_t nz = (uint32_t)((size_t)((char*)sh.dn - (char*)sh.cdiff) / 16);   // cdiff, ex, del, oth, deficit
             for (uint32_t i = tid; i < nz; i += TL_THREADS) z[i] = make_uint4(0, 0, 0, 0);
             // ... and the tile's chain heads in HBM: only this tile's walks insert at its positions (push_other), so the 4 B per
             // position that a call has to zero are zeroed here, by the CTA that is about to use them, not by a memset over the assembly
@@ -1354,35 +1432,61 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
 #ifdef PP_TILE_PROF
         pt[3] = clock64();
 #endif
-        // ---- phase C: difference arrays -> cover / multi per position
+        // ---- phase C: difference arrays -> cover per position, and the deficit where alignments with k != 1 touch the tile.  After
+        // the scans every thread only reads and writes its own positions of `deficit` / `depth`: no barrier until the end of the tile.
         const uint32_t rel0 = tid * TL_PER_THREAD;
-        uint32_t cover[TL_PER_THREAD], multi[TL_PER_THREAD];
+        uint32_t cover[TL_PER_THREAD];
+        uint32_t multi = 0;                                  // bit i: position rel0 + i has k != 1 coverage (depth from the deficit)
         {
-            long long csum = 0, msum = 0;
+            long long csum = 0;
 #pragma unroll
-            for (int i = 0; i < TL_PER_THREAD; ++i) { csum += sh.cdiff[rel0 + i]; msum += sh.mdiff[rel0 + i]; cover[i] = (uint32_t)csum; multi[i] = (uint32_t)msum; }
-            // both sums in one scan: cover + 2^32 * multi as ONE signed 64-bit integer.  A thread's own sum can be negative, but
-            // every prefix of both sums is non-negative (and cover < 2^32), so the exclusive prefix decodes uniquely.
-            const unsigned long long packed = (unsigned long long)(csum + (msum << 32));
-            const unsigned long long ex = block_exscan<TL_THREADS>(packed, sh.s_warp, &sh.s_total);
-            uint32_t anym = 0;
+            for (int i = 0; i < TL_PER_THREAD; ++i) { csum += sh.cdiff[rel0 + i]; cover[i] = (uint32_t)csum; }
+            const unsigned long long ex = block_exscan<TL_THREADS>((unsigned long long)csum, sh.s_warp, &sh.s_total);
 #pragma unroll
-            for (int i = 0; i < TL_PER_THREAD; ++i) { cover[i] += (uint32_t)ex; multi[i] += (uint32_t)(ex >> 32); anym |= multi[i]; }
-            if (anym) atomicOr(&sh.subflags, 1u << (rel0 >> PP_SUB_SHIFT));
+            for (int i = 0; i < TL_PER_THREAD; ++i) cover[i] += (uint32_t)ex;
+            if (sh.any_multi) {                              // (block-uniform)
+                unsigned long long dsum = 0, dv[TL_PER_THREAD];
+#pragma unroll
+                for (int i = 0; i < TL_PER_THREAD; ++i) { dsum += sh.deficit[rel0 + i]; dv[i] = dsum; }
+                const unsigned long long dex = block_exscan<TL_THREADS>(dsum, sh.s_warp, &sh.s_total);
+#pragma unroll
+                for (int i = 0; i < TL_PER_THREAD; ++i) {
+                    sh.deficit[rel0 + i] = dv[i] + dex;
+                    if (dv[i] + dex != 0 || cover[i] >= TL_DEF_COVER) multi |= 1u << i;
+                }
+            }
         }
-        __syncthreads();
 #ifdef PP_TILE_PROF
         pt[4] = clock64();
 #endif
-        // ---- phase D: ordered depth where a sub-tile sees k != 1.  Warp w owns sub-tile w here AND in the vote below, so there is
-        // no block-wide barrier in between: warps of unflagged sub-tiles go straight on.
+        // ---- phase D: the ordered depth walk, where the deficit's bound cannot settle the vote.  Warp w owns sub-tile w here AND in
+        // the vote below.  A position decides the vote without depth when no allele other than the draft's can reach the valid
+        // threshold (the same tests as in phase E, on the lower bound), else when both ends of the bound give the same thresholds.
+        // The debug records print depth itself: there every sub-tile with k != 1 coverage walks.
+        bool walk;
+        {
+            bool open = false;
+            if (multi && !vp.dbg) {
+#pragma unroll
+                for (int i = 0; i < TL_PER_THREAD; ++i) {
+                    if (!((multi >> i) & 1u)) continue;
+                    const uint32_t rel = rel0 + i;
+                    if (cover[i] >= TL_DEF_COVER) { open = true; continue; }
+                    const uint32_t mx = max(max(max(sh.ex[0][rel], sh.ex[1][rel]), max(sh.ex[2][rel], sh.ex[3][rel])), max(sh.del[rel], sh.oth[rel]));
+                    if (mx == 0 || mx < prm.min_depth) continue;
+                    const DepthBounds db = depth_bounds(cover[i], sh.deficit[rel]);
+                    if ((double)mx + 2.0 < db.lo * prm.fv) continue;
+                    if (!same_thresholds(prm, db.lo, db.hi)) open = true;
+                }
+            }
+            walk = __ballot_sync(0xffffffffu, vp.dbg ? multi != 0 : open) != 0;
+        }
 #ifdef PP_TILE_PROF
         const long long dw0 = clock64();
 #endif
-        if ((sh.subflags >> warp) & 1u) depth_walk<BITS>(d, sh, sh.wstage[warp], P0, warp, lb, long_lo, long_hi);
+        if (walk) depth_walk<BITS>(d, sh, sh.wstage[warp], P0, warp, lb, long_lo, long_hi);
 #ifdef PP_TILE_PROF
-        if (lane == 0 && ((sh.subflags >> warp) & 1u)) { atomicAdd(&d.st->prof[8], (unsigned long long)(clock64() - dw0)); atomicAdd(&d.st->prof[9], 1ull); }
-        if (tid == 0 && sh.subflags) atomicAdd(&d.st->prof[10], 1ull);
+        if (lane == 0 && walk) { atomicAdd(&d.st->prof[8], (unsigned long long)(clock64() - dw0)); atomicAdd(&d.st->prof[9], 1ull); }
 #endif
         __syncwarp();
         // ---- phase E: the vote, straight out of shared memory
@@ -1429,7 +1533,14 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 continue;
             }
             const uint32_t rel = rel0 + i;
-            const double depth = multi[i] ? sh.depth[rel] : (double)cov;
+            // depth: the reference's where it is known (no k != 1 coverage, or the warp walked), else the fixed-point estimate
+            // (per-contig statistics only).  vdepth, what the vote reads: there the lower bound, whose thresholds phase D found
+            // to be the reference's.
+            double depth = (double)cov, vdepth = depth;
+            if ((multi >> i) & 1u) {
+                if (walk) depth = vdepth = sh.depth[rel];
+                else { const DepthBounds db = depth_bounds(cov, sh.deficit[rel]); depth = db.fx; vdepth = db.lo; }
+            }
             tdepth += depth;
             uint32_t cA = sh.ex[0][rel], cC = sh.ex[1][rel], cG = sh.ex[2][rel], cT = sh.ex[3][rel];
             const uint32_t cDel = sh.del[rel], n_other = sh.oth[rel];
@@ -1446,7 +1557,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 // non-draft count is below min_depth, or below depth * fraction_valid by more than rounding can bridge: the
                 // position keeps its base whatever its status (kept / too_close / low_depth / none / multiple).
                 const uint32_t mx = max(max(max(cA, cC), max(cG, cT)), max(cDel, n_other));
-                if (mx < prm.min_depth || (double)mx + 2.0 < depth * prm.fv) {
+                if (mx < prm.min_depth || (double)mx + 2.0 < vdepth * prm.fv) {
                     po[i].packed = (orig == '-' ? 0u : 1u) | (orig << 16);
                     tlen += po[i].packed & 0xFFFFu;
                     continue;
@@ -1457,7 +1568,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             else if (orig == 'C') { cC += matched; matched = 0; }
             else if (orig == 'G') { cG += matched; matched = 0; }
             else if (orig == 'T') { cT += matched; matched = 0; }
-            po[i] = vote_position<BITS>(oc, prm, p, orig, depth, cA, cC, cG, cT, cDel, matched, n_other, vp.dbg ? vp.dbg + p : nullptr);
+            po[i] = vote_position<BITS>(oc, prm, p, orig, vdepth, cA, cC, cG, cT, cDel, matched, n_other, vp.dbg ? vp.dbg + p : nullptr);
             n_changed += (po[i].packed >> 24) & 1u;
             tlen += po[i].packed & 0xFFFFu;
         }
@@ -1492,6 +1603,9 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         long long delta = (long long)tlen - (long long)npos;
         for (int o = 16; o > 0; o >>= 1) delta += __shfl_down_sync(0xffffffffu, delta, o);
         if (lane == 0) sh.s_delta[warp] = delta;
+#ifdef PP_TILE_PROF
+        if (__syncthreads_or(walk) && tid == 0) atomicAdd(&d.st->prof[10], 1ull);
+#endif
         __syncthreads();
         if (tid == 0) {
             long long t = 0;
