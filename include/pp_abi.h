@@ -190,6 +190,23 @@ int pp_polish_debug_fetch(pp_ctx* ctx, uint64_t first_pos, uint64_t n_pos, pp_de
 /* head[p] = 1 + index of the first node of global position p (0 = none); nodes[0..*n_nodes) */
 int pp_polish_debug_alleles(pp_ctx* ctx, uint32_t* head /* [total bp] */, pp_debug_node* nodes, uint64_t node_cap, uint64_t* n_nodes);
 
+/* The change report (--changes): the --debug record of every position whose status is changed (pileup.rs:156-163), and nothing
+ * for the others.  Recording is off by default; unlike pp_polish_set_debug it keeps the vote's shortcuts and costs one record per
+ * changed position.  Switch it on before the polish call (1 record, 2 stop recording but keep the last rows, 0 off).  The number of
+ * rows of a call is the sum of its pp_polish_result.changed. */
+int pp_polish_set_changes(pp_ctx* ctx, int on);
+/* The rows of the last polish with recording on, in position order: pos[i] its global position (contig offset + position in the
+ * contig), rows[i] its record, pool + pool_off[i] its allele strings: uint32 n, n times (uint32 count, uint32 length, the characters)
+ * for every allele other than A, C, G, T, "-" and the draft's own base, then uint32 length and the characters of the emitted allele
+ * when it is one of those (rows[i].new_node != 0xFFFFFFFF; length 0 otherwise); integers little-endian, unaligned.  *n_rows and
+ * *pool_bytes are always set: call once with row_cap = pool_cap = 0 (and NULL buffers) for the sizes, then with the buffers. */
+int pp_polish_changes_fetch(pp_ctx* ctx, uint64_t row_cap, uint64_t* pos, pp_debug_pos* rows, uint64_t* pool_off, uint8_t* pool,
+                            uint64_t pool_cap, uint64_t* n_rows, uint64_t* pool_bytes);
+/* The whole-command calls below (pp_polish_files, pp_polish_files_multi, pp_filter_polish_files) made with `ctx` (ctxs[0]) as
+ * their context also write the change report to `path`: the --debug header line, then the --debug rows whose status is changed,
+ * in the assembly's contig order and position order.  NULL or "" switches it off (the default).  The path is copied. */
+int pp_set_changes_file(pp_ctx* ctx, const char* path);
+
 /* ------------------------------------------------------------------------------------------------------
  * filter (filter.rs).  One record per ALIGNED line of one mate's SAM file, in file order.
  * Replaces get_insert_size_thresholds (filter.rs:148-186) and alignment_pass_qc (filter.rs:352-377).

@@ -60,6 +60,12 @@ class PolishResult(C.Structure):
                 ("error_aln", C.c_int64), ("timing", Timing)]
 
 
+class DebugPos(C.Structure):
+    _fields_ = [("depth", C.c_double), ("valid_threshold", C.c_uint32), ("invalid_threshold", C.c_uint32), ("count", C.c_uint32 * 6),
+                ("n_other", C.c_uint32), ("new_node", C.c_uint32), ("original", C.c_uint8), ("status", C.c_uint8), ("new_char", C.c_uint8),
+                ("pad", C.c_uint8 * 5)]
+
+
 class FilterMate(C.Structure):
     _fields_ = [("n", C.c_uint64), ("name_id", C.c_void_p), ("contig", C.c_void_p), ("ref_start", C.c_void_p),
                 ("ref_end", C.c_void_p), ("flags", C.c_void_p)]
@@ -148,6 +154,10 @@ def lib():
     L.pp_tok_set_strip_qual.argtypes = [C.c_void_p, C.c_int]
     L.pp_dataset_sizes.argtypes = [C.c_void_p, C.POINTER(Alignments)]
     L.pp_dataset_download.argtypes = [C.c_void_p, C.POINTER(Alignments)]
+    L.pp_polish_set_changes.argtypes = [C.c_void_p, C.c_int]
+    L.pp_set_changes_file.argtypes = [C.c_void_p, C.c_char_p]
+    L.pp_polish_changes_fetch.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                          C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     if hasattr(L, "pp_filter"):
         L.pp_filter.argtypes = [C.c_void_p, C.POINTER(FilterMate), C.POINTER(FilterMate), C.POINTER(FilterParams),
                                 C.POINTER(FilterResult)]
@@ -364,24 +374,67 @@ class Context:
         self._nc = contigs.n_contigs
         self._G = int(np.ctypeslib.as_array(C.cast(contigs.off, C.POINTER(C.c_uint64)), shape=(contigs.n_contigs + 1,))[-1])
 
-    def polish_resident(self, fetch=True, **opts):
+    def polish_resident(self, fetch=True, changes=False, **opts):
+        """pp_polish_resident.  changes=True: the call also records the change report, returned under "changes" (changes_rows)."""
         prm = _params(**opts)
         cap = self._G + (1 << 20) if fetch else 0
-        for _ in range(2):
-            if fetch:
-                res, keep = self._result(self._nc, cap)
-            else:
-                res, keep = PolishResult(), None
-            rc = lib().pp_polish_resident(self.h, C.byref(prm), C.byref(res))
-            if fetch and rc == PP_ERR_ARG and res.out_len > cap:
-                cap = int(res.out_len)
-                continue
-            break
+        L = lib()
+        if changes:
+            L.pp_polish_set_changes(self.h, 1)
+        ok = False
+        try:
+            for _ in range(2):
+                if fetch:
+                    res, keep = self._result(self._nc, cap)
+                else:
+                    res, keep = PolishResult(), None
+                rc = L.pp_polish_resident(self.h, C.byref(prm), C.byref(res))
+                if fetch and rc == PP_ERR_ARG and res.out_len > cap:
+                    cap = int(res.out_len)
+                    continue
+                break
+            if rc != PP_OK:
+                raise self._err(rc)
+            ok = True
+        finally:
+            if changes:
+                L.pp_polish_set_changes(self.h, 2 if ok else 0)     # a failed call leaves nothing recording
+        out = self._finish(res, keep, self._nc) if fetch else dict(n_aln_used=res.n_aln_used, out_len=res.out_len, timing=res.timing.as_dict())
+        if changes:
+            out["changes"] = self.changes_rows()
+        return out
+
+    def changes_rows(self):
+        """The change report of the last polish with changes recorded (pp_polish_changes_fetch), in position order: one dict per
+        changed position with its global position, its pp_debug_pos fields, its other alleles [(string, count)] and the emitted
+        allele as a string."""
+        L = lib()
+        n, nb = C.c_uint64(), C.c_uint64()
+        rc = L.pp_polish_changes_fetch(self.h, 0, None, None, None, None, 0, C.byref(n), C.byref(nb))
         if rc != PP_OK:
             raise self._err(rc)
-        if not fetch:
-            return dict(n_aln_used=res.n_aln_used, out_len=res.out_len, timing=res.timing.as_dict())
-        return self._finish(res, keep, self._nc)
+        pos, off = np.zeros(max(1, n.value), np.uint64), np.zeros(max(1, n.value), np.uint64)
+        recs = (DebugPos * max(1, n.value))()
+        pool = np.zeros(max(1, nb.value), np.uint8)
+        rc = L.pp_polish_changes_fetch(self.h, n.value, pos.ctypes.data, C.addressof(recs), off.ctypes.data, pool.ctypes.data, nb.value,
+                                       C.byref(n), C.byref(nb))
+        if rc != PP_OK:
+            raise self._err(rc)
+        raw = pool.tobytes()
+        rows = []
+        for i in range(n.value):
+            r = recs[i]
+            q = int(off[i])
+            alleles = []
+            for _ in range(int.from_bytes(raw[q:q + 4], "little")):
+                cnt, ln = int.from_bytes(raw[q + 4:q + 8], "little"), int.from_bytes(raw[q + 8:q + 12], "little")
+                alleles.append((raw[q + 12:q + 12 + ln].decode("latin-1"), cnt))
+                q += 8 + ln
+            ln = int.from_bytes(raw[q + 4:q + 8], "little")
+            new = raw[q + 8:q + 8 + ln].decode("latin-1") if r.new_node != 0xFFFFFFFF else chr(r.new_char)
+            rows.append(dict(pos=int(pos[i]), depth=r.depth, valid=r.valid_threshold, invalid=r.invalid_threshold, count=list(r.count),
+                             original=chr(r.original), status=r.status, alleles=alleles, new_base=new))
+        return rows
 
     # ---- device SAM tokeniser (tok_kernels.cu) ------------------------------------------------------------------
     def tokenise(self, fasta, sources, careful=False, seq_bits=4):
@@ -456,29 +509,42 @@ class Context:
         lib().pp_set_parser(self.h, int(mode))
 
     # ---- file level (what the CLI does) ----------------------------------------------------------------------
-    def polish_files(self, assembly, sams, debug=None, verbose=False, **opts):
+    def set_changes_file(self, path):
+        """pp_set_changes_file: the file-level calls on this context also write the change report to `path` (None: off)."""
+        lib().pp_set_changes_file(self.h, str(path).encode() if path else None)
+
+    def polish_files(self, assembly, sams, debug=None, changes=None, verbose=False, **opts):
         prm = _params(**opts)
         arr = (C.c_char_p * max(1, len(sams)))(*[str(s).encode() for s in sams])
         out = C.c_void_p()
         n = C.c_uint64()
-        rc = lib().pp_polish_files(self.h, str(assembly).encode(), arr, len(sams), C.byref(prm),
-                                   str(debug).encode() if debug else None, C.byref(out), C.byref(n), int(verbose))
+        self.set_changes_file(changes)
+        try:
+            rc = lib().pp_polish_files(self.h, str(assembly).encode(), arr, len(sams), C.byref(prm),
+                                       str(debug).encode() if debug else None, C.byref(out), C.byref(n), int(verbose))
+        finally:
+            self.set_changes_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
         lib().pp_free(out)
         return data
 
-    def filter_polish_files(self, assembly, in1, in2, out1=None, out2=None, orientation="auto", low=0.1, high=99.9, verbose=False, **opts):
+    def filter_polish_files(self, assembly, in1, in2, out1=None, out2=None, orientation="auto", low=0.1, high=99.9, verbose=False, changes=None,
+                            **opts):
         """pp_filter_polish_files: `filter` then `polish` in one call (the filtered SAM files are written only when named)."""
         L = lib()
         L.pp_filter_polish_files.argtypes = [C.c_void_p] + [C.c_char_p] * 6 + [C.c_double, C.c_double, C.POINTER(PolishParams),
                                                                               C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
         prm = _params(**opts)
         out, n = C.c_void_p(), C.c_uint64()
-        rc = L.pp_filter_polish_files(self.h, str(assembly).encode(), str(in1).encode(), str(in2).encode(),
-                                      str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
-                                      low, high, C.byref(prm), C.byref(out), C.byref(n), int(verbose))
+        self.set_changes_file(changes)
+        try:
+            rc = L.pp_filter_polish_files(self.h, str(assembly).encode(), str(in1).encode(), str(in2).encode(),
+                                          str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
+                                          low, high, C.byref(prm), C.byref(out), C.byref(n), int(verbose))
+        finally:
+            self.set_changes_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
@@ -498,9 +564,10 @@ def polish_files(assembly, sams, device=0, **kw):
 
 
 def polish(assembly, sam, debug=None, fraction_invalid=0.2, fraction_valid=0.5, max_errors=10, min_depth=5,
-           careful=False, device=0):
-    """`polypolish polish` (main.rs:78-108, polish.rs:26-38): returns the bytes the reference prints to stdout."""
-    return polish_files(assembly, list(sam), device=device, debug=debug, fraction_invalid=fraction_invalid,
+           careful=False, device=0, changes=None):
+    """`polypolish polish` (main.rs:78-108, polish.rs:26-38): returns the bytes the reference prints to stdout.  changes: also
+    write the change report (the --debug rows of the changed positions) to this file."""
+    return polish_files(assembly, list(sam), device=device, debug=debug, changes=changes, fraction_invalid=fraction_invalid,
                         fraction_valid=fraction_valid, max_errors=max_errors, min_depth=min_depth, careful=careful)
 
 
@@ -698,10 +765,11 @@ class TwoBit:
             pass
 
 
-def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, contexts=None, **opts):
+def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, contexts=None, changes=None, **opts):
     """pp_polish_files_multi: contigs shard over one context per entry of `devices` (entries may repeat), or over the given `contexts`
     (reused across calls like a long-running host would).  parser 0 (default): every context tokenises the text itself and keeps its
-    shard (pp_tok_set_shard); 1: host packer + host sharder."""
+    shard (pp_tok_set_shard); 1: host packer + host sharder.  changes: also write the change report to this file (every context
+    reports its own contigs)."""
     L = lib()
     L.pp_polish_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_char_p, C.POINTER(C.c_char_p), C.c_int,
                                         C.POINTER(PolishParams), C.c_char_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
@@ -712,8 +780,12 @@ def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, co
         prm = _params(**opts)
         arr = (C.c_char_p * max(1, len(sams)))(*[str(s).encode() for s in sams])
         out, n = C.c_void_p(), C.c_uint64()
-        rc = L.pp_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), arr, len(sams), C.byref(prm), None,
-                                     C.byref(out), C.byref(n), int(verbose))
+        ctxs[0].set_changes_file(changes)
+        try:
+            rc = L.pp_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), arr, len(sams), C.byref(prm), None,
+                                         C.byref(out), C.byref(n), int(verbose))
+        finally:
+            ctxs[0].set_changes_file(None)
         if rc != PP_OK:
             raise ctxs[0]._err(rc)
         data = C.string_at(out, n.value)

@@ -6,7 +6,8 @@
 //                     [-d|--min_depth 5] [--careful] <ASSEMBLY> [SAM]...
 // Polished FASTA on stdout, log on stderr, "Error: <msg>" + exit 1 on user errors (misc.rs:29-33).
 // Additive flags: --device N (first GPU), --gpus N (polish: contigs shard across N GPUs), --quiet, --host-parse (polish: parse the
-// SAM text on the host instead of on the device; same output).  All compute happens in libpolypolish_b200.so on the GPU.
+// SAM text on the host instead of on the device; same output), --changes F (polish, filter-polish: the --debug rows of the changed
+// positions only).  All compute happens in libpolypolish_b200.so on the GPU.
 #include <cstdio>
 #include <unistd.h>
 #include <cstdlib>
@@ -85,7 +86,8 @@ static void help_polish() {               // main.rs:77-108
     puts("          Print help");
     puts("  -V, --version");
     puts("          Print version");
-    puts("\nH100 build, additive options: --device <N> (first GPU, default 0), --gpus <N> (contigs shard over N GPUs), --quiet, --host-parse");
+    puts("\nH100 build, additive options: --device <N> (first GPU, default 0), --gpus <N> (contigs shard over N GPUs), --quiet, --host-parse, "
+         "--changes <FILE> (the --debug rows of the changed positions only)");
 }
 
 // clap accepts `--name=value`, `-m5` / `-m=5` and a `--` separator (everything after it is positional): normalise those forms
@@ -157,7 +159,7 @@ struct Args {
     std::vector<Token> tok;
     size_t i = 0;
     pp_polish_params prm{0.2, 0.5, 10, 5, 0};
-    std::string debug, in1, in2, out1, out2, orientation = "auto";
+    std::string debug, changes, in1, in2, out1, out2, orientation = "auto";
     double low = 0.1, high = 99.9;
     int device = 0, gpus = 1;
     bool quiet = false, host_parse = false;
@@ -168,9 +170,10 @@ struct Args {
     }
 };
 
-// -i / -v / -m / -d / --careful of `polish` and `filter-polish`
+// -i / -v / -m / -d / --careful / --changes of `polish` and `filter-polish`
 static bool polish_option(const std::string& a, Args& g) {
-    if (a == "-i" || a == "--fraction_invalid") g.prm.fraction_invalid = parse_f64("--fraction_invalid <FRACTION_INVALID>", g.value("--fraction_invalid"));
+    if (a == "--changes") g.changes = g.value("--changes <FILE>");
+    else if (a == "-i" || a == "--fraction_invalid") g.prm.fraction_invalid = parse_f64("--fraction_invalid <FRACTION_INVALID>", g.value("--fraction_invalid"));
     else if (a == "-v" || a == "--fraction_valid") g.prm.fraction_valid = parse_f64("--fraction_valid <FRACTION_VALID>", g.value("--fraction_valid"));
     else if (a == "-m" || a == "--max_errors") g.prm.max_errors = parse_u32("--max_errors <MAX_ERRORS>", g.value("--max_errors"));
     else if (a == "-d" || a == "--min_depth") g.prm.min_depth = parse_u32("--min_depth <MIN_DEPTH>", g.value("--min_depth"));
@@ -222,6 +225,7 @@ static std::vector<pp_ctx*> open_contexts(const Args& g) {
         if (pp_create(base + d, &ctxs[d]) != PP_OK) quit_with_error("no usable H100 (sm_90) GPU: this build has no CPU fallback");
     mark("contexts created");
     if (g.host_parse) pp_set_parser(ctxs[0], 1);
+    if (!g.changes.empty()) pp_set_changes_file(ctxs[0], g.changes.c_str());
     return ctxs;
 }
 

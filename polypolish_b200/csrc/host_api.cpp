@@ -19,6 +19,7 @@
 #include <utility>
 #include <vector>
 
+#include "debug_rows.h"
 #include "pp_internal.h"
 
 namespace {
@@ -37,90 +38,33 @@ std::string qscore_text(double identity) {
 
 extern "C" void pp_free(void* p) { free(p); }
 
-// misc.rs:170-182 complement_base (upper-case input)
-static char complement_char(char b) {
-    switch (b) {
-        case 'A': return 'T'; case 'T': return 'A'; case 'G': return 'C'; case 'C': return 'G'; case 'N': return 'N';
-        case 'R': return 'Y'; case 'Y': return 'R'; case 'S': return 'S'; case 'W': return 'W'; case 'K': return 'M'; case 'M': return 'K';
-        case 'B': return 'V'; case 'V': return 'B'; case 'D': return 'H'; case 'H': return 'D';
-        case '.': return '.'; case '-': return '-'; case '?': return '?';
-        default: return 'N';
-    }
-}
-
-// The string of one "other" allele node (pileup.rs:62 key).
-static std::string node_allele(const pp_debug_node& nd, const pp_alignments* a) {
-    static const char* NIB = "=ACMGRSVTWYHKDBN";
-    std::string out;
-    if (a->seq_bits == 4 && (nd.sig & 15)) {
-        for (uint32_t i = 0; i < (nd.sig & 15); ++i) out += NIB[(nd.sig >> (4 * (i + 1))) & 15];
-        return out;
-    }
-    if (a->seq_bits == 8 && (nd.sig & 255)) {
-        for (uint32_t i = 0; i < (nd.sig & 255); ++i) out += (char)((nd.sig >> (8 * (i + 1))) & 255);
-        return out;
-    }
-    const uint32_t aln = (uint32_t)(nd.val >> 32), start = (uint32_t)(nd.val >> 16) & 0xFFFFu, len = (uint32_t)nd.val & 0xFFFFu;
-    const bool rc = a->flags[aln] & PP_FLAG_RC;
-    const uint32_t n = a->seq_len[aln];
-    for (uint32_t i = 0; i < len; ++i) {
-        const uint32_t e = start + i, j = rc ? (n - 1 - e) : e;
-        char ch;
-        if (a->seq_bits == 4) {
-            const uint8_t b = a->seq_pool[(size_t)a->seq_off[aln] * (PP_SEQ_BLOCK / 2) + (j >> 1)];
-            ch = NIB[(b >> ((j & 1) * 4)) & 15];
-        } else {
-            ch = (char)a->seq_pool[(size_t)a->seq_off[aln] * PP_SEQ_BLOCK + j];
-        }
-        out += rc ? complement_char(ch) : ch;
-    }
-    return out;
-}
-
-// write_debug_header / write_debug_line (polish.rs:247-266) + get_debug_line / get_count_str (pileup.rs:137-166)
-static int write_debug_tsv(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs* contigs, const pp_alignments* alns, FILE* f) {
-    static const char* STATUS[6] = {"low_depth", "none", "multiple", "too_close", "kept", "changed"};
-    const uint64_t G = contigs->off[contigs->n_contigs];
-    std::vector<uint32_t> head(G);
-    uint64_t n_nodes = 0;
-    pp_polish_debug_alleles(ctx, nullptr, nullptr, 0, &n_nodes);           // size query (reports the node count, then fails on the null buffers)
-    std::vector<pp_debug_node> nodes(n_nodes + 1);
-    int rc = pp_polish_debug_alleles(ctx, head.data(), nodes.data(), n_nodes, &n_nodes);
-    if (rc != PP_OK) return rc;
-    if (fputs("name\tpos\tbase\tdepth\tinvalid\tvalid\tpileup\tstatus\tnew_base\n", f) < 0) return PP_ERR_IO;
+// write_debug_header / write_debug_line (polish.rs:247-266): every position of the assembly, one chunk at a time; the allele strings
+// of the positions that have other alleles come from the device (k_allele_strings)
+static int write_debug_tsv(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs* contigs, FILE* f) {
+    if (fputs(pp::DEBUG_HEADER, f) < 0) return PP_ERR_IO;
     const uint64_t CH = 1 << 18;
     std::vector<pp_debug_pos> recs(CH);
+    std::vector<uint32_t> at;
+    std::vector<uint64_t> off;
+    std::vector<uint8_t> pool;
+    pp::DebugRows rows;
     std::string buf;
-    std::vector<std::string> counts;
-    char tmp[64];
     for (uint32_t c = 0; c < contigs->n_contigs; ++c) {
         const char* name = pp_fasta_name(fa, c);
         for (uint64_t p0 = contigs->off[c]; p0 < contigs->off[c + 1]; p0 += CH) {
             const uint64_t n = std::min<uint64_t>(CH, contigs->off[c + 1] - p0);
-            rc = pp_polish_debug_fetch(ctx, p0, n, recs.data());
+            int rc = pp_polish_debug_fetch(ctx, p0, n, recs.data());
+            if (rc != PP_OK) return rc;
+            at.clear();
+            for (uint64_t i = 0; i < n; ++i)
+                if (recs[i].n_other || recs[i].new_node != 0xFFFFFFFFu) at.push_back((uint32_t)(p0 + i));
+            rc = pp_polish_debug_strings(ctx, at.data(), (uint32_t)at.size(), off, pool);
             if (rc != PP_OK) return rc;
             buf.clear();
+            size_t k = 0;
             for (uint64_t i = 0; i < n; ++i) {
-                const pp_debug_pos& r = recs[i];
-                const uint64_t gp = p0 + i;
-                counts.clear();
-                static const char* ACGT = "ACGT";
-                for (int b = 0; b < 4; ++b) if (r.count[b]) counts.push_back(std::string(1, ACGT[b]) + "x" + std::to_string(r.count[b]));
-                if (r.count[4]) counts.push_back("-x" + std::to_string(r.count[4]));
-                if (r.count[5]) counts.push_back(std::string(1, (char)r.original) + "x" + std::to_string(r.count[5]));
-                for (uint32_t nd = head[gp]; nd != 0;) {
-                    const pp_debug_node& node = nodes[nd - 1];
-                    counts.push_back(node_allele(node, alns) + "x" + std::to_string(node.count));
-                    nd = node.next == 0xFFFFFFFFu ? 0 : node.next + 1;
-                }
-                std::sort(counts.begin(), counts.end());
-                buf += name; buf += '\t'; buf += std::to_string(gp - contigs->off[c]); buf += '\t'; buf += (char)r.original; buf += '\t';
-                snprintf(tmp, sizeof tmp, "%.1f", r.depth);          // Rust {:.1}: both round the exact binary value
-                buf += tmp; buf += '\t'; buf += std::to_string(r.invalid_threshold); buf += '\t'; buf += std::to_string(r.valid_threshold); buf += '\t';
-                for (size_t k = 0; k < counts.size(); ++k) { if (k) buf += ','; buf += counts[k]; }
-                buf += '\t'; buf += STATUS[r.status < 6 ? r.status : 0]; buf += '\t';
-                if (r.new_node != 0xFFFFFFFFu) buf += node_allele(nodes[r.new_node], alns); else buf += (char)r.new_char;
-                buf += '\n';
+                const uint8_t* al = (k < at.size() && at[k] == p0 + i) ? pool.data() + off[k++] : nullptr;
+                rows.add(buf, name, p0 + i - contigs->off[c], recs[i], al);
             }
             if (fwrite(buf.data(), 1, buf.size(), f) != buf.size()) return PP_ERR_IO;
         }
@@ -170,26 +114,6 @@ static void run_shard(ShardJob* j, const pp_polish_params* prm) {
     }
     if (j->rc != PP_OK) j->err = pp_last_error(j->ctx);
 }
-
-// The resident dataset of a context copied back into host arrays (pp_dataset_download).  Plain new[] without value
-// initialisation: the copy overwrites every byte, so zero-filling 0.4 GB first would only cost time.
-struct HostCopy {
-    std::unique_ptr<uint32_t[]> contig, ref_start, read_id, seq_off, cigar_off, nm, cigar_ops;
-    std::unique_ptr<uint16_t[]> seq_len, n_cigar;
-    std::unique_ptr<uint8_t[]> flags, seq_pool;
-    int fetch(pp_ctx* ctx, pp_alignments* v) {
-        int rc = pp_dataset_sizes(ctx, v);
-        if (rc != PP_OK) return rc;
-        const size_t n = (size_t)v->n_aln + 1;
-        contig.reset(new uint32_t[n]); ref_start.reset(new uint32_t[n]); read_id.reset(new uint32_t[n]); seq_off.reset(new uint32_t[n]);
-        cigar_off.reset(new uint32_t[n]); nm.reset(new uint32_t[n]); seq_len.reset(new uint16_t[n]); n_cigar.reset(new uint16_t[n]);
-        flags.reset(new uint8_t[n]); cigar_ops.reset(new uint32_t[(size_t)v->n_cigar_ops + 1]); seq_pool.reset(new uint8_t[(size_t)v->seq_pool_bytes + 64]);
-        v->contig = contig.get(); v->ref_start = ref_start.get(); v->read_id = read_id.get(); v->seq_off = seq_off.get();
-        v->cigar_off = cigar_off.get(); v->nm = nm.get(); v->seq_len = seq_len.get(); v->n_cigar = n_cigar.get(); v->flags = flags.get();
-        v->cigar_ops = cigar_ops.get(); v->seq_pool = seq_pool.get();
-        return pp_dataset_download(ctx, v);
-    }
-};
 
 // Cuts a SAM file into n byte ranges for n GPUs: cut[0] = 0, cut[n] = size, every other cut is the start of a line whose QNAME differs from
 // the line before it (a read group - consecutive lines of one QNAME, alignment.rs:214-272 - is never split).  false: not a plain file,
@@ -262,20 +186,21 @@ using FastaPtr = std::unique_ptr<pp_fasta, Deleter<pp_fasta_free>>;
 using PackPtr = std::unique_ptr<pp_pack, Deleter<pp_pack_free>>;
 using ShardsPtr = std::unique_ptr<pp_shards, Deleter<pp_shards_free>>;
 
-// --debug: the context records per-position debug data for the length of the call.  It is left in mode 2 (not recording, the
-// records of this call readable) when the call succeeded, otherwise in mode 0, so that later calls neither record nor read stale data.
-struct DebugRecording {
-    pp_ctx* ctx;
-    bool on, ok = false;
-    DebugRecording(pp_ctx* c, bool o) : ctx(c), on(o) { if (on) pp_polish_set_debug(ctx, 1); }
-    ~DebugRecording() { if (on) pp_polish_set_debug(ctx, ok ? 2 : 0); }
+// --debug / --changes: the contexts record per-position data (Set = pp_polish_set_debug / pp_polish_set_changes) for the length of
+// the call.  They are left in mode 2 (not recording, the records of this call readable) when the call succeeded, otherwise in mode
+// 0, so that later calls neither record nor read stale data.
+template <int (*Set)(pp_ctx*, int)>
+struct Recording {
+    std::vector<pp_ctx*> ctxs;
+    bool ok = false;
+    Recording(pp_ctx* const* c, int n, bool on) { if (on) for (int i = 0; i < n; ++i) { ctxs.push_back(c[i]); Set(c[i], 1); } }
+    ~Recording() { for (pp_ctx* c : ctxs) Set(c, ok ? 2 : 0); }
 };
 
 // What one way of loading the alignments leaves for the polish: one job per GPU, whatever backs their arrays, and what to print.
 struct Load {
     std::vector<ShardJob> jobs;
-    pp_alignments alns{};                // all alignments; host arrays only when `copy` or `pack` backs them (n_aln always)
-    HostCopy copy;                       // the tokenised arrays back on the host (--debug: allele strings of the TSV)
+    pp_alignments alns{};                // all alignments; host arrays only when `pack` backs them (n_aln always)
     PackPtr pack;
     ShardsPtr shards;
     std::string log, timing;             // the reference's per-file lines (alignment.rs:266-271); timing lines
@@ -434,7 +359,7 @@ static int tokenise(const pp_fasta* fa, const char* const* sams, int n_sams, int
 // The device tokeniser: one GPU reads the whole files; several each take their own contigs and a byte range of every file.
 // PP_OK, PP_TOK_HOST or an error.
 static int load_device(pp_ctx* const* ctxs, uint32_t n, const pp_fasta* fa, const pp_contigs& contigs, const char* const* sams, int n_sams,
-                       int careful, bool debug, Load& ld) {
+                       int careful, Load& ld) {
     std::vector<uint32_t> owner;
     std::vector<std::vector<uint64_t>> cuts;
     if (n > 1) {
@@ -444,10 +369,7 @@ static int load_device(pp_ctx* const* ctxs, uint32_t n, const pp_fasta* fa, cons
     }
     for (int i = 0; i < n_sams; ++i) cuts.push_back({0, pp::file_size(sams[i])});
     one_job(ld, ctxs[0], contigs, true);
-    int rc = tokenise(fa, sams, n_sams, careful, cuts, owner, contigs.n_contigs, ld);
-    const uint64_t n_aln = ld.alns.n_aln;                                     // (the alignments the tokeniser read)
-    if (rc == PP_OK && debug) rc = ld.copy.fetch(ctxs[0], &ld.alns);         // the allele strings of the debug TSV
-    ld.alns.n_aln = n_aln;
+    const int rc = tokenise(fa, sams, n_sams, careful, cuts, owner, contigs.n_contigs, ld);
     ld.jobs[0].alns = ld.alns;
     return rc;
 }
@@ -554,6 +476,39 @@ static std::string assemble(const pp_fasta* fa, const pp_contigs& contigs, const
     return out;
 }
 
+// --changes: the --debug rows of the changed positions, in the input FASTA's contig order, then position order.  Every job reports
+// the rows of its own contigs (pp_polish_changes_fetch); they are merged here.  PP_ERR_IO: the file could not be written; another
+// error: its message is on ctx.
+static int write_changes(pp_ctx* ctx, const pp_fasta* fa, const std::vector<ShardJob>& jobs, FILE* f) {
+    struct Fetched { std::vector<uint64_t> pos, off; std::vector<pp_debug_pos> rows; std::vector<uint8_t> pool; };
+    struct Row { uint32_t contig; uint64_t pos; uint32_t job; uint64_t i; };
+    std::vector<Fetched> got(jobs.size());
+    std::vector<Row> order;
+    for (uint32_t s = 0; s < jobs.size(); ++s) {
+        const ShardJob& j = jobs[s];
+        Fetched& g = got[s];
+        uint64_t n = 0, bytes = 0;
+        int rc = pp_polish_changes_fetch(j.ctx, 0, nullptr, nullptr, nullptr, nullptr, 0, &n, &bytes);
+        if (rc == PP_OK) {
+            g.pos.resize(n); g.off.resize(n); g.rows.resize(n); g.pool.resize(bytes);
+            rc = pp_polish_changes_fetch(j.ctx, n, g.pos.data(), g.rows.data(), g.off.data(), g.pool.data(), bytes, &n, &bytes);
+        }
+        if (rc != PP_OK) return pp_ctx_fail(ctx, rc, std::string(pp_last_error(j.ctx)).c_str());
+        for (uint64_t i = 0; i < n; ++i) {             // global position in the job's own assembly -> (input contig, position in it)
+            const uint32_t lc = (uint32_t)(std::upper_bound(j.contigs.off, j.contigs.off + j.contigs.n_contigs + 1, g.pos[i]) - j.contigs.off) - 1;
+            order.push_back({jobs.size() == 1 ? lc : j.contig_map[lc], g.pos[i] - j.contigs.off[lc], s, i});
+        }
+    }
+    std::sort(order.begin(), order.end(), [](const Row& a, const Row& b) { return a.contig != b.contig ? a.contig < b.contig : a.pos < b.pos; });
+    std::string buf = pp::DEBUG_HEADER;
+    pp::DebugRows rows;
+    for (const Row& r : order) {
+        const Fetched& g = got[r.job];
+        rows.add(buf, pp_fasta_name(fa, r.contig), r.pos, g.rows[r.i], g.pool.data() + g.off[r.i]);
+    }
+    return fwrite(buf.data(), 1, buf.size(), f) == buf.size() ? PP_OK : PP_ERR_IO;
+}
+
 static void print_timing(const Load& ld) {
     fputs(ld.timing.c_str(), stderr);
     for (uint32_t s = 0; s < ld.jobs.size(); ++s) {
@@ -588,8 +543,16 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
         debug_file = fopen(debug_path, "wb");
         if (!debug_file) return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + std::string(debug_path) + "\"").c_str());
     }
-    struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file};
-    DebugRecording recording(ctx, debug);
+    const std::string changes_path = pp_ctx_changes_file(ctx);
+    const bool changes = !changes_path.empty();
+    FILE* changes_file = nullptr;
+    if (changes) {                                        // worded like --debug's
+        changes_file = fopen(changes_path.c_str(), "wb");
+        if (!changes_file) { if (debug_file) fclose(debug_file); return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + changes_path + "\"").c_str()); }
+    }
+    struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file}, closer2{changes_file};
+    Recording<pp_polish_set_debug> recording(&ctx, 1, debug);
+    Recording<pp_polish_set_changes> recording_changes(ctxs, n_ctx, changes);
 
     // the first SAM file starts streaming into HBM while the assembly is loaded
     const bool device_parser = pp_get_parser(ctx) == 0;
@@ -614,7 +577,7 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     int rc = PP_TOK_HOST;
     if (device_parser && (ff || n_sams > 0)) {
         rc = ff ? load_fused(ctx, fa.get(), contigs, sams, *ff, prm->careful, ld)
-                : load_device(ctxs, n_shards, fa.get(), contigs, sams, n_sams, prm->careful, debug, ld);
+                : load_device(ctxs, n_shards, fa.get(), contigs, sams, n_sams, prm->careful, ld);
         if (rc == PP_OK) run_jobs(ld.jobs, prm);
         if (rc == PP_OK && data_error(ld.jobs)) rc = PP_TOK_HOST;
         if (rc == PP_OK && verbose) fputs(ld.log.c_str(), stderr);
@@ -635,11 +598,15 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     }
     if (rc == PP_OK) rc = job_error(ctx, ld);
     if (rc == PP_OK && debug) {
-        rc = write_debug_tsv(ctx, fa.get(), &contigs, &ld.alns, debug_file);
+        rc = write_debug_tsv(ctx, fa.get(), &contigs, debug_file);
         if (rc != PP_OK && rc != PP_ERR_CUDA) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + std::string(debug_path) + "\"").c_str());
     }
+    if (rc == PP_OK && changes) {
+        rc = write_changes(ctx, fa.get(), ld.jobs, changes_file);
+        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + changes_path + "\"").c_str());
+    }
     if (rc != PP_OK) return rc;
-    recording.ok = true;
+    recording.ok = recording_changes.ok = true;
     if (verbose) {
         uint64_t n_used = 0;
         for (const ShardJob& j : ld.jobs) n_used += j.res.n_aln_used;

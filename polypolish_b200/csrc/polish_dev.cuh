@@ -68,7 +68,8 @@ struct DevStatus {
     unsigned int flags;
     unsigned int max_ext;            // (binning) largest entry count of a binned alignment: how many bins a tile looks back
     unsigned int ticket;             // next tile (k_tile's dynamic schedule)
-    unsigned int pad0, pad1;
+    unsigned int n_changes;          // changed positions k_tile appended to the change list (counted beyond its capacity too)
+    unsigned int pad1;
 #ifdef PP_TILE_PROF
     unsigned long long prof[12];     // cycles of thread 0 per phase (A, B, queue, C, D+E), queued reads, tiles, largest queue, depth-walk cycles, walks, tiles with a walk
 #endif
@@ -666,6 +667,13 @@ struct VoteParams {
     uint32_t* rec_at;                 // [G] other-allele node to emit at a position (only where res says so)
     long long* chunk_delta;           // [n_chunks] sum(output length) - positions of the chunk
     pp_debug_pos* dbg;                // [G] per-position debug records, or nullptr
+    // --changes: the record of every position whose status is changed, appended in no particular order, or nullptr.  Only such
+    // positions can emit another base than the draft's, and every one of them reaches the vote (the shortcuts skip only positions
+    // that keep their base), so the list costs one atomic per changed position.
+    pp_debug_pos* chg;                // [chg_cap]
+    uint32_t* chg_pos;                // [chg_cap] global position of each record
+    unsigned int* chg_n;              // records appended (DevStatus::n_changes); more than chg_cap: the list overflowed
+    uint32_t chg_cap;
 };
 
 // What the other-allele slow path needs, passed by value so that the kernel parameter structs are never
@@ -705,11 +713,23 @@ __device__ __forceinline__ uint8_t other_char(const OthCtx& oc, uint32_t rec, ui
 // multi-base node), bit 24 changed, bit 25 emit from node `rec`.
 struct PosOut { uint32_t packed; uint32_t rec; };
 
-// The vote of pileup.rs:67-134 for one covered position.  packed bits 26..28 carry the BaseStatus.
-template <int BITS>
+// The debug record of one voted position (what get_debug_line prints, pileup.rs:137-166).
+__device__ __forceinline__ void debug_record(pp_debug_pos* r, double depth, uint32_t vt, uint32_t it, uint32_t cA, uint32_t cC, uint32_t cG,
+                                             uint32_t cT, uint32_t cDel, uint32_t matched, uint32_t n_other, uint32_t orig, uint32_t status, PosOut o) {
+    r->depth = depth; r->valid_threshold = vt; r->invalid_threshold = it;
+    r->count[0] = cA; r->count[1] = cC; r->count[2] = cG; r->count[3] = cT; r->count[4] = cDel; r->count[5] = matched;
+    r->n_other = n_other;
+    r->new_node = ((o.packed >> 25) & 1u) ? o.rec : 0xFFFFFFFFu;
+    r->original = (uint8_t)orig; r->status = (uint8_t)status;
+    r->new_char = ((o.packed >> 25) & 1u) ? 0 : (((o.packed & 0xFFFFu) == 0 && orig != '-') ? (uint8_t)'-' : (uint8_t)(o.packed >> 16));
+}
+
+// The vote of pileup.rs:67-134 for one covered position.  packed bits 26..28 carry the BaseStatus.  `depth` must be the
+// reference's own where a record is written (vp.dbg, or CHG and the position changes): the records print it.
+template <int BITS, bool CHG>
 __device__ __forceinline__ PosOut vote_position(const OthCtx& oc, const DevParams& prm, uint32_t pos, uint32_t orig, double depth,
                                                 uint32_t cA, uint32_t cC, uint32_t cG, uint32_t cT, uint32_t cDel,
-                                                uint32_t matched, uint32_t n_other, pp_debug_pos* dbg) {
+                                                uint32_t matched, uint32_t n_other, const VoteParams& vp) {
     const Thresholds th = vote_thresholds(prm, depth);
     const uint32_t vt = th.vt, it = th.it;
     Tally t{0, 0, -1, 0};
@@ -748,13 +768,13 @@ __device__ __forceinline__ PosOut vote_position(const OthCtx& oc, const DevParam
         }
     }
     o.packed |= status << 26;
-    if (dbg) {
-        dbg->depth = depth; dbg->valid_threshold = vt; dbg->invalid_threshold = it;
-        dbg->count[0] = cA; dbg->count[1] = cC; dbg->count[2] = cG; dbg->count[3] = cT; dbg->count[4] = cDel; dbg->count[5] = matched;
-        dbg->n_other = n_other;
-        dbg->new_node = ((o.packed >> 25) & 1u) ? o.rec : 0xFFFFFFFFu;
-        dbg->original = (uint8_t)orig; dbg->status = (uint8_t)status;
-        dbg->new_char = ((o.packed >> 25) & 1u) ? 0 : (((o.packed & 0xFFFFu) == 0 && orig != '-') ? (uint8_t)'-' : (uint8_t)(o.packed >> 16));
+    if (vp.dbg) debug_record(vp.dbg + pos, depth, vt, it, cA, cC, cG, cT, cDel, matched, n_other, orig, status, o);
+    if (CHG && status == 5) {
+        const uint32_t slot = atomicAdd(vp.chg_n, 1u);
+        if (slot < vp.chg_cap) {
+            vp.chg_pos[slot] = pos;
+            debug_record(vp.chg + slot, depth, vt, it, cA, cC, cG, cT, cDel, matched, n_other, orig, status, o);
+        }
     }
     return o;
 }
@@ -1288,7 +1308,10 @@ __device__ __forceinline__ void depth_walk(const DevData& d, TileShared& sh, Wal
     } else depth_walk_steps<BITS>(d, sh, P0, sub, lb, long_lo, long_hi);
 }
 
-template <int BITS>
+// CHG: the change report is recorded (vp.chg; without it the vp.chg* fields are not read).  A template argument, so that the kernel
+// without the report does the work it did before the report existed (as a run-time test it measured up to 0.5 % slower on an H100,
+// 700 W, 5 Mbp x 100x).
+template <int BITS, bool CHG = false>
 __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp, TileShared& sh) {
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const DevParams prm = *d.prm;
@@ -1462,7 +1485,8 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         // ---- phase D: the ordered depth walk, where the deficit's bound cannot settle the vote.  Warp w owns sub-tile w here AND in
         // the vote below.  A position decides the vote without depth when no allele other than the draft's can reach the valid
         // threshold (the same tests as in phase E, on the lower bound), else when both ends of the bound give the same thresholds.
-        // The debug records print depth itself: there every sub-tile with k != 1 coverage walks.
+        // The debug records print depth itself: there every sub-tile with k != 1 coverage walks.  The change records print it too:
+        // there a sub-tile also walks when one of its positions passes these tests, which every position that reaches the vote does.
         bool walk;
         {
             bool open = false;
@@ -1476,7 +1500,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                     if (mx == 0 || mx < prm.min_depth) continue;
                     const DepthBounds db = depth_bounds(cover[i], sh.deficit[rel]);
                     if ((double)mx + 2.0 < db.lo * prm.fv) continue;
-                    if (!same_thresholds(prm, db.lo, db.hi)) open = true;
+                    if (CHG || !same_thresholds(prm, db.lo, db.hi)) open = true;
                 }
             }
             walk = __ballot_sync(0xffffffffu, vp.dbg ? multi != 0 : open) != 0;
@@ -1568,7 +1592,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             else if (orig == 'C') { cC += matched; matched = 0; }
             else if (orig == 'G') { cG += matched; matched = 0; }
             else if (orig == 'T') { cT += matched; matched = 0; }
-            po[i] = vote_position<BITS>(oc, prm, p, orig, vdepth, cA, cC, cG, cT, cDel, matched, n_other, vp.dbg ? vp.dbg + p : nullptr);
+            po[i] = vote_position<BITS, CHG>(oc, prm, p, orig, vdepth, cA, cC, cG, cT, cDel, matched, n_other, vp);
             n_changed += (po[i].packed >> 24) & 1u;
             tlen += po[i].packed & 0xFFFFu;
         }
@@ -1626,10 +1650,61 @@ static_assert(TL_PER_THREAD == 4, "the verdict store packs four positions per th
 #if !defined(PP_EMULATE)
 // One CTA per SM: built for sm_90a, the body needs ~100 registers per thread.  Capped at 64 for two CTAs per SM it spills, and on an
 // H100 (400 W) the tile kernel took 0.79 ms per 5 Mbp x 100x call that way against 0.71 ms with one CTA per SM.
-template <int BITS>
+template <int BITS, bool CHG>
 __global__ void __launch_bounds__(TL_THREADS, 1) k_tile(DevData d, VoteParams vp) {
     extern __shared__ __align__(16) unsigned char tile_smem[];
-    tile_body<BITS>(d, vp, *reinterpret_cast<TileShared*>(tile_smem));
+    tile_body<BITS, CHG>(d, vp, *reinterpret_cast<TileShared*>(tile_smem));
+}
+#endif
+
+// ------------------------------------------------------------------------------------------------------
+// k_allele_strings: the strings behind debug and change records (the keys of the reference's HashMap<String,u32>, pileup.rs:62),
+// so that a report never needs the alignments on the host.  Runs after a polish call, on its chains.  Row i (global position
+// pos[i], record rec[by_pos ? pos[i] : i]) gets, at pool + off[i]: u32 n, then n times (u32 count, u32 length, the characters)
+// for the position's other alleles in chain order, then u32 length and the characters of the emitted allele when that is a node
+// (length 0 otherwise); little-endian.  Space is taken with one atomicAdd per row on *used: where *used ends above cap, rows were
+// left unwritten and the call is repeated with a pool of *used bytes.
+// ------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint8_t* put_u32(uint8_t* w, uint32_t v) {
+    w[0] = (uint8_t)v; w[1] = (uint8_t)(v >> 8); w[2] = (uint8_t)(v >> 16); w[3] = (uint8_t)(v >> 24);
+    return w + 4;
+}
+template <int BITS>
+__device__ void allele_strings_row(const OthCtx& oc, uint32_t pos, uint32_t new_node, uint8_t* pool, unsigned long long cap,
+                                   unsigned long long* used, unsigned long long* off) {
+    unsigned long long bytes = 8;
+    uint32_t n = 0;
+    for (uint32_t nd = oc.head[pos]; nd != 0; nd = oc.nodes[nd - 1].next == NONE32 ? 0 : oc.nodes[nd - 1].next + 1) {
+        bytes += 8 + ((uint32_t)oc.nodes[nd - 1].val & 0xFFFFu);
+        n++;
+    }
+    const uint32_t new_len = new_node == NONE32 ? 0u : (uint32_t)oc.nodes[new_node].val & 0xFFFFu;
+    bytes += new_len;
+    const unsigned long long o = atomicAdd(used, bytes);
+    *off = o;
+    if (o + bytes > cap) return;
+    uint8_t* w = put_u32(pool + o, n);
+    for (uint32_t nd = oc.head[pos]; nd != 0; nd = oc.nodes[nd - 1].next == NONE32 ? 0 : oc.nodes[nd - 1].next + 1) {
+        const uint32_t len = (uint32_t)oc.nodes[nd - 1].val & 0xFFFFu;
+        w = put_u32(put_u32(w, oc.nodes[nd - 1].count), len);
+        for (uint32_t t = 0; t < len; ++t) *w++ = other_char<BITS>(oc, nd - 1, t);
+    }
+    w = put_u32(w, new_len);
+    for (uint32_t t = 0; t < new_len; ++t) *w++ = other_char<BITS>(oc, new_node, t);
+}
+template <int BITS>
+__device__ void allele_strings_body(const OthCtx& oc, const uint32_t* pos, const pp_debug_pos* rec, bool by_pos, uint32_t n, uint8_t* pool,
+                                    unsigned long long cap, unsigned long long* used, unsigned long long* off) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t p = pos[i];
+        allele_strings_row<BITS>(oc, p, rec[by_pos ? p : i].new_node, pool, cap, used, off + i);
+    }
+}
+#if !defined(PP_EMULATE)
+template <int BITS>
+__global__ void __launch_bounds__(256) k_allele_strings(OthCtx oc, const uint32_t* pos, const pp_debug_pos* rec, bool by_pos, uint32_t n,
+                                                         uint8_t* pool, unsigned long long cap, unsigned long long* used, unsigned long long* off) {
+    allele_strings_body<BITS>(oc, pos, rec, by_pos, n, pool, cap, used, off);
 }
 #endif
 

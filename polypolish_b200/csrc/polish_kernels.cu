@@ -379,13 +379,16 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
     const uint64_t G = ctx->G, n_aln = ctx->n_aln;
     const uint32_t n_tiles = (uint32_t)((G + TL_T - 1) / TL_T);              // = vote / compaction chunks
     const size_t padG = (size_t)n_tiles * TL_T + 16;                          // k_tile / k_compact move whole chunks with vector accesses
+    ctx->have_changes = false;
 
     CK(ctx->b[B_OUTOFF].ensure(((size_t)ctx->n_contigs + 1) * 8));
     CK(ctx->b[B_RES].ensure(padG * 2)); CK(ctx->b[B_RECAT].ensure((G + 1) * 4)); CK(ctx->b[B_CHUNKDELTA].ensure((size_t)n_tiles * 8));
     CK(ctx->b[B_PARAMS].ensure(sizeof(DevParams)));
     if (!ctx->tile_attr_set) {
-        CK(cudaFuncSetAttribute(k_tile<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
         ctx->tile_attr_set = true;
     }
 
@@ -455,11 +458,18 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
         vp.chunk_delta = ctx->b[B_CHUNKDELTA].as<long long>();
         vp.dbg = nullptr;
         if (ctx->debug_on) { CK(ctx->b[B_DEBUG].ensure((G + 1) * sizeof(pp_debug_pos))); vp.dbg = ctx->b[B_DEBUG].as<pp_debug_pos>(); }
+        vp.chg = nullptr; vp.chg_pos = nullptr; vp.chg_n = &d.st->n_changes; vp.chg_cap = 0;
+        if (ctx->changes_on) {
+            if (ctx->chg_cap == 0) ctx->chg_cap = (uint32_t)std::max<uint64_t>(4096, G / 256);
+            CK(ctx->b[B_CHG].ensure((size_t)ctx->chg_cap * sizeof(pp_debug_pos))); CK(ctx->b[B_CHGPOS].ensure((size_t)ctx->chg_cap * 4));
+            vp.chg = ctx->b[B_CHG].as<pp_debug_pos>(); vp.chg_pos = ctx->b[B_CHGPOS].as<uint32_t>(); vp.chg_cap = ctx->chg_cap;
+        }
         {
             int occ = 1;
-            CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_tile<BITS>, TL_THREADS, sizeof(TileShared)));
+            CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vp.chg ? k_tile<BITS, true> : k_tile<BITS, false>, TL_THREADS, sizeof(TileShared)));
             const uint32_t grid = std::min<uint32_t>(n_tiles, (uint32_t)ctx->sm_count * (uint32_t)std::max(occ, 1));   // persistent: tiles by ticket
-            k_tile<BITS><<<grid, TL_THREADS, sizeof(TileShared), s>>>(d, vp);
+            if (vp.chg) k_tile<BITS, true><<<grid, TL_THREADS, sizeof(TileShared), s>>>(d, vp);
+            else k_tile<BITS, false><<<grid, TL_THREADS, sizeof(TileShared), s>>>(d, vp);
             ctx->launches++;
         }
         // ---- stage 4: compaction
@@ -487,9 +497,12 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
         if (hs.flags & FL_BIGGROUP) { if (ctx->global_k) return ctx->fail(PP_ERR_CUDA, "internal error: FL_BIGGROUP in global-k mode"); ctx->global_k = true; again = true; }
         if (hs.flags & FL_NODE_OVF) { ctx->node_cap = (uint32_t)std::min<uint64_t>(0x7FFFFFFFull, (uint64_t)hs.node_count + hs.node_count / 4 + 1024); again = true; }
         if (!again && (hs.flags & FL_OUT_OVF)) { ctx->out_cap = hs.out_len + 64; again = true; }
+        // the change list: its exact length is the number of changed positions, counted past the end (= the sum of `changed`)
+        if (!again && ctx->changes_on && hs.n_changes > ctx->chg_cap) { ctx->chg_cap = hs.n_changes; again = true; }
         if (again) continue;
 
         ctx->have_debug = ctx->debug_on; ctx->last_head = d.oth_head; ctx->last_nodes = std::min(hs.node_count, node_cap);
+        ctx->have_changes = ctx->changes_on; ctx->n_changes = ctx->changes_on ? hs.n_changes : 0; ctx->chg_pool = -1;
         res->out_len = hs.out_len;
         res->n_aln_used = hs.n_used;
         res->error_aln = -1;
@@ -589,5 +602,98 @@ extern "C" int pp_polish_debug_alleles(pp_ctx* ctx, uint32_t* head, pp_debug_nod
     CK(cudaMemcpyAsync(head, ctx->last_head, ctx->G * 4, cudaMemcpyDeviceToHost, ctx->stream));
     if (ctx->last_nodes) CK(cudaMemcpyAsync(nodes, ctx->b[B_NODES].p, (size_t)ctx->last_nodes * sizeof(OthNode), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
+    return PP_OK;
+}
+
+// k_allele_strings over n rows of the last call (positions pos_dev, records rec_dev) into B_STRPOOL / B_STROFF; *bytes = pool bytes.
+template <int BITS>
+static int allele_strings(pp_ctx* ctx, const uint32_t* pos_dev, const pp_debug_pos* rec_dev, bool by_pos, uint32_t n, uint64_t* bytes) {
+    cudaStream_t s = ctx->stream;
+    OthCtx oc;
+    oc.nodes = ctx->b[B_NODES].as<OthNode>(); oc.head = ctx->last_head;
+    oc.sr = SeqRef{ctx->b[B_SEQPOOL].as<uint8_t>(), ctx->b[B_SEQOFF].as<uint32_t>(), ctx->b[B_SEQLEN].as<uint16_t>(), ctx->b[B_FLAGS].as<uint8_t>()};
+    CK(ctx->b[B_STROFF].ensure((size_t)n * 8 + 8));
+    unsigned long long* used = ctx->b[B_STROFF].as<unsigned long long>() + n;                 // (behind the offsets)
+    uint64_t cap = std::max<uint64_t>(ctx->b[B_STRPOOL].cap, (uint64_t)n * 16 + 4096);
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        CK(ctx->b[B_STRPOOL].ensure(cap));
+        CK(cudaMemsetAsync(used, 0, 8, s));
+        if (n) k_allele_strings<BITS><<<(n + 255) / 256, 256, 0, s>>>(oc, pos_dev, rec_dev, by_pos, n, ctx->b[B_STRPOOL].as<uint8_t>(), cap, used, ctx->b[B_STROFF].as<unsigned long long>());
+        CK(cudaMemcpyAsync(bytes, used, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        CK(cudaGetLastError());
+        if (*bytes <= cap) return PP_OK;
+        cap = *bytes;                                                     // the exact size: the second round fits
+    }
+    return ctx->fail(PP_ERR_NOMEM, "allele strings: pool kept overflowing");
+}
+static int allele_strings(pp_ctx* ctx, const uint32_t* pos_dev, const pp_debug_pos* rec_dev, bool by_pos, uint32_t n, uint64_t* bytes) {
+    return ctx->seq_bits == 4 ? allele_strings<4>(ctx, pos_dev, rec_dev, by_pos, n, bytes) : allele_strings<8>(ctx, pos_dev, rec_dev, by_pos, n, bytes);
+}
+
+// internal (host_api.cpp): the allele strings of the --debug records at n positions (pp_polish_set_debug), in k_allele_strings' format
+int pp_polish_debug_strings(pp_ctx* ctx, const uint32_t* pos, uint32_t n, std::vector<uint64_t>& off, std::vector<uint8_t>& pool) {
+    if (!ctx->have_debug || !ctx->last_head) return ctx->fail(PP_ERR_ARG, "pp_polish_debug_strings: no debug polish on this context");
+    CK(cudaSetDevice(ctx->device));
+    CK(ctx->b[B_STRPOS].ensure((size_t)n * 4 + 4));
+    if (n) CK(cudaMemcpyAsync(ctx->b[B_STRPOS].p, pos, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    uint64_t bytes = 0;
+    const int rc = allele_strings(ctx, ctx->b[B_STRPOS].as<uint32_t>(), ctx->b[B_DEBUG].as<pp_debug_pos>(), true, n, &bytes);
+    if (rc != PP_OK) return rc;
+    off.resize(n);
+    pool.resize(bytes);
+    if (n) CK(cudaMemcpyAsync(off.data(), ctx->b[B_STROFF].p, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (bytes) CK(cudaMemcpyAsync(pool.data(), ctx->b[B_STRPOOL].p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    return PP_OK;
+}
+
+extern "C" int pp_polish_set_changes(pp_ctx* ctx, int on) {
+    if (!ctx) return PP_ERR_ARG;
+    ctx->changes_on = on == 1;          // 2 = stop recording but keep the last call's rows readable
+    if (on == 0) ctx->have_changes = false;
+    return PP_OK;
+}
+
+extern "C" int pp_set_changes_file(pp_ctx* ctx, const char* path) {
+    if (!ctx) return PP_ERR_ARG;
+    ctx->changes_path = path ? path : "";
+    return PP_OK;
+}
+const char* pp_ctx_changes_file(pp_ctx* ctx) { return ctx->changes_path.c_str(); }
+
+extern "C" int pp_polish_changes_fetch(pp_ctx* ctx, uint64_t row_cap, uint64_t* pos, pp_debug_pos* rows, uint64_t* pool_off, uint8_t* pool,
+                                       uint64_t pool_cap, uint64_t* n_rows, uint64_t* pool_bytes) {
+    if (!ctx) return PP_ERR_ARG;
+    if (!ctx->have_changes || !ctx->last_head) return ctx->fail(PP_ERR_ARG, "pp_polish_changes_fetch: the last polish did not record changes (pp_polish_set_changes)");
+    if (!n_rows || !pool_bytes) return ctx->fail(PP_ERR_ARG, "pp_polish_changes_fetch: null size pointers");
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t n = ctx->n_changes;
+    if (ctx->chg_pool < 0) {
+        uint64_t bytes = 0;
+        const int rc = allele_strings(ctx, ctx->b[B_CHGPOS].as<uint32_t>(), ctx->b[B_CHG].as<pp_debug_pos>(), false, n, &bytes);
+        if (rc != PP_OK) return rc;
+        ctx->chg_pool = (int64_t)bytes;
+    }
+    *n_rows = n;
+    *pool_bytes = (uint64_t)ctx->chg_pool;
+    if (row_cap == 0 && pool_cap == 0 && n > 0) return PP_OK;                                 // size query
+    if (row_cap < n || pool_cap < *pool_bytes || (n && (!pos || !rows || !pool_off || !pool)))
+        return ctx->fail(PP_ERR_ARG, "pp_polish_changes_fetch: buffers too small");
+    // the rows arrive in the order the tiles appended them: sorted by position here, the pool stays as it is
+    std::vector<uint32_t> p(n);
+    std::vector<pp_debug_pos> r(n);
+    std::vector<uint64_t> o(n);
+    if (n) {
+        CK(cudaMemcpyAsync(p.data(), ctx->b[B_CHGPOS].p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(r.data(), ctx->b[B_CHG].p, (size_t)n * sizeof(pp_debug_pos), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(o.data(), ctx->b[B_STROFF].p, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    if (*pool_bytes) CK(cudaMemcpyAsync(pool, ctx->b[B_STRPOOL].p, *pool_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::vector<uint32_t> order(n);
+    for (uint32_t i = 0; i < n; ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return p[a] < p[b]; });
+    for (uint32_t i = 0; i < n; ++i) { pos[i] = p[order[i]]; rows[i] = r[order[i]]; pool_off[i] = o[order[i]]; }
     return PP_OK;
 }
