@@ -125,12 +125,18 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
 
 }  // namespace
 
+static int g_last_global_k = 0;
+
+// Whether the last emu_polish repeated itself in global-k mode (a read group too large for k_goodk's in-block count).
+extern "C" int emu_last_global_k() { return g_last_global_k; }
+
 // The polish kernels on the CPU.  grid_tiles = CTAs of k_tile (they share tiles through the ticket, like on the device).
 extern "C" int emu_polish(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,
                           unsigned long long* err_code) {
     init_comp_table();
     uint64_t err = 0;
     int rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, false, &err) : run<8>(c, a, prm, res, grid_tiles, false, &err);
+    g_last_global_k = rc == 100;
     if (rc == 100) rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, true, &err) : run<8>(c, a, prm, res, grid_tiles, true, &err);
     if (err_code) *err_code = err;
     return rc;
