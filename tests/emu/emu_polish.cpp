@@ -8,6 +8,9 @@
 #include <numeric>
 #include <string>
 
+static int g_last_global_k = 0;
+static unsigned g_last_max_ext = 0, g_last_n_long = 0;
+
 namespace {
 
 void init_comp_table() {
@@ -80,6 +83,8 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
     emu::launch((unsigned)((n_aln + 1 + 255) / 256), 256, 0, [&] { bin_bounds_body(skey.data(), (uint32_t)n_aln, n_bins + 2, bin_start.data()); });
     d.n_slots = bin_start[n_bins + 1];
     d.max_ext = st.max_ext;
+    g_last_max_ext = st.max_ext;
+    g_last_n_long = bin_start[n_bins + 1] - bin_start[n_bins];
     if (d.n_slots) {
         emu::launch((d.n_slots + 255) / 256, 256, 0, [&] { permute_body(d); });
         if (BITS == 4) emu::launch((unsigned)(((uint64_t)d.n_slots * TL_SEQ_QUADS + 255) / 256), 256, 0, [&] { permute_seq_body(d); });
@@ -125,10 +130,12 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
 
 }  // namespace
 
-static int g_last_global_k = 0;
-
 // Whether the last emu_polish repeated itself in global-k mode (a read group too large for k_goodk's in-block count).
 extern "C" int emu_last_global_k() { return g_last_global_k; }
+// What the last emu_polish binned: the largest entry count of a binned alignment (max_ext: a tile looks (max_ext + 255) / 256 bins
+// back) and the alignments of the long list.
+extern "C" unsigned emu_last_max_ext() { return g_last_max_ext; }
+extern "C" unsigned emu_last_n_long() { return g_last_n_long; }
 
 // The polish kernels on the CPU.  grid_tiles = CTAs of k_tile (they share tiles through the ticket, like on the device).
 extern "C" int emu_polish(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,

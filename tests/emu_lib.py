@@ -60,7 +60,7 @@ def polish(fasta, packed, grid_tiles=2, **opts):
     off = keep["off"]
     return dict(sequences=[keep["bases"][int(off[i]):int(off[i + 1])].tobytes() for i in range(n)], changed=keep["changed"].tolist(),
                 zero_depth=keep["zero"].tolist(), total_depth=keep["tdepth"].tolist(), n_aln_used=res.n_aln_used,
-                global_k=bool(lib().emu_last_global_k()))
+                global_k=bool(lib().emu_last_global_k()), max_ext=lib().emu_last_max_ext(), n_long=lib().emu_last_n_long())
 
 
 def fasta_bytes(fasta, seqs):
