@@ -385,6 +385,20 @@ int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, const char* o
 int pp_filter_polish_files(pp_ctx* ctx, const char* assembly, const char* in1, const char* in2, const char* out1, const char* out2,
                            const char* orientation, double low, double high, const pp_polish_params* params, char** out_fasta,
                            uint64_t* out_len, int verbose);
+/* `polypolish filter` over several GPUs of one box (filter.rs:26-37: load_alignments :91-145, get_insert_size_thresholds :148-186,
+ * alignment_pass_qc :352-377, filter_sam :296-349).  GPU g reads byte range g of both files (pp_sam_split_ranges), every record travels to
+ * the GPU that owns its read name (the verdict depends only on the alignments that share it), the pair counts and the percentiles are
+ * reduced across GPUs, and each GPU writes its piece of both output files.  Same bytes, messages and log numbers as pp_filter_files;
+ * anything that path does not settle (host parsing asked for, an input that is not a regular file, what pp_filter_files_device would
+ * leave to the host) runs as pp_filter_files on ctxs[0].  n_ctx == 1 is pp_filter_files. */
+int pp_filter_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                          const char* orientation, double low, double high, int verbose);
+/* pp_filter_polish_files over several GPUs (filter::filter then polish::polish, polish.rs:26-38): the filter as in pp_filter_files_multi,
+ * then every GPU tokenises its ranges with its verdicts as ZP flags and the read groups move to their contigs' GPUs as in
+ * pp_polish_files_multi.  More than 32 contexts, and anything that path does not settle, run as pp_filter_polish_files on ctxs[0]. */
+int pp_filter_polish_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* assembly, const char* in1, const char* in2, const char* out1,
+                                 const char* out2, const char* orientation, double low, double high, const pp_polish_params* params,
+                                 char** out_fasta, uint64_t* out_len, int verbose);
 void pp_free(void* p);
 
 /* ------------------------------------------------------------------------------------------------------

@@ -795,3 +795,54 @@ def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, co
         if contexts is None:
             for c in ctxs:
                 c.close()
+
+
+def _with_contexts(devices, contexts, parser, fn):
+    ctxs = contexts if contexts is not None else [Context(d) for d in devices]
+    try:
+        ctxs[0].set_parser(parser)
+        return fn(ctxs, (C.c_void_p * len(ctxs))(*[c.h for c in ctxs]))
+    finally:
+        if contexts is None:
+            for c in ctxs:
+                c.close()
+
+
+def filter_files_multi(in1, in2, out1, out2, orientation="auto", low=0.1, high=99.9, devices=None, verbose=False, parser=0, contexts=None):
+    """pp_filter_files_multi: `polypolish filter` with one context per entry of `devices` (entries may repeat) or over the given
+    `contexts`: each filters a byte range of both SAM files, the records meet on the context that owns their read name."""
+    L = lib()
+    L.pp_filter_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int] + [C.c_char_p] * 5 + [C.c_double, C.c_double, C.c_int]
+
+    def run(ctxs, arr_ctx):
+        rc = L.pp_filter_files_multi(arr_ctx, len(ctxs), str(in1).encode(), str(in2).encode(), str(out1).encode(), str(out2).encode(),
+                                     orientation.encode(), low, high, int(verbose))
+        if rc != PP_OK:
+            raise ctxs[0]._err(rc)
+    _with_contexts(devices, contexts, parser, run)
+
+
+def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientation="auto", low=0.1, high=99.9, devices=None, verbose=False,
+                              parser=0, contexts=None, changes=None, **opts):
+    """pp_filter_polish_files_multi: `filter` then `polish` in one call over one context per entry of `devices` (entries may repeat) or
+    over the given `contexts`; the filtered SAM files are written only when named.  changes: also write the change report to this file."""
+    L = lib()
+    L.pp_filter_polish_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int] + [C.c_char_p] * 6 + [
+        C.c_double, C.c_double, C.POINTER(PolishParams), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
+    prm = _params(**opts)
+
+    def run(ctxs, arr_ctx):
+        out, n = C.c_void_p(), C.c_uint64()
+        ctxs[0].set_changes_file(changes)
+        try:
+            rc = L.pp_filter_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), str(in1).encode(), str(in2).encode(),
+                                                str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
+                                                low, high, C.byref(prm), C.byref(out), C.byref(n), int(verbose))
+        finally:
+            ctxs[0].set_changes_file(None)
+        if rc != PP_OK:
+            raise ctxs[0]._err(rc)
+        data = C.string_at(out, n.value)
+        L.pp_free(out)
+        return data
+    return _with_contexts(devices, contexts, parser, run)

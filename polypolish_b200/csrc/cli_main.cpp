@@ -5,7 +5,8 @@
 //   polypolish polish [--debug F] [-i|--fraction_invalid 0.2] [-v|--fraction_valid 0.5] [-m|--max_errors 10]
 //                     [-d|--min_depth 5] [--careful] <ASSEMBLY> [SAM]...
 // Polished FASTA on stdout, log on stderr, "Error: <msg>" + exit 1 on user errors (misc.rs:29-33).
-// Additive flags: --device N (first GPU), --gpus N (polish: contigs shard across N GPUs), --quiet, --host-parse (polish: parse the
+// Additive flags: --device N (first GPU), --gpus N (polish: contigs shard across N GPUs), --gpu-count N (filter, filter-polish: each of N
+// GPUs filters a byte range of both SAM files; `filter` and `filter-polish` keep rejecting --gpus, as they always have), --quiet, --host-parse (polish: parse the
 // SAM text on the host instead of on the device; same output), --changes F (polish, filter-polish: the --debug rows of the changed
 // positions only).  All compute happens in libpolypolish_b200.so on the GPU.
 #include <cstdio>
@@ -60,7 +61,8 @@ static void help_filter() {               // main.rs:46-75
     puts("      --high <HIGH>                High percentile threshold [default: 99.9]");
     puts("  -h, --help                       Print help");
     puts("  -V, --version                    Print version");
-    puts("\nH100 build, additive options: --device <N> (GPU, default 0), --quiet, --host-parse");
+    puts("\nH100 build, additive options: --device <N> (first GPU, default 0), --gpu-count <N> (each of N GPUs filters a byte range of both "
+         "files), --quiet, --host-parse");
 }
 
 static void help_polish() {               // main.rs:77-108
@@ -195,8 +197,15 @@ static bool filter_option(const std::string& a, Args& g) {
     return true;
 }
 
+// --gpu-count of `filter` and `filter-polish`: GPUs [device, device + N), each filtering (and tokenising) a byte range of both files
+static bool gpu_count_option(const std::string& a, Args& g) {
+    if (a != "--gpu-count") return false;
+    g.gpus = (int)parse_u32("--gpu-count <N>", g.value("--gpu-count <N>"));
+    return true;
+}
+
 // The option loop of every subcommand: `own(a, g)` handles the subcommand's own flags (true: handled), then come --device, --gpus
-// (when `gpus`), --quiet and --host-parse.  Positionals are collected when `positionals`, else they are clap's "unexpected argument".
+// (when `gpus`), --quiet and --host-parse.  `filter` and `filter-polish` take their GPU count as --gpu-count (their own flag).  Positionals are collected when `positionals`, else they are clap's "unexpected argument".
 template <class F>
 static Args parse_args(int argc, char** argv, const char* value_shorts, bool positionals, bool gpus, F&& own) {
     Args g;
@@ -271,14 +280,14 @@ int main(int argc, char** argv) {
         Args g = parse_args(argc, argv, "", false, false, [](const std::string& a, Args& g) {
             if (a == "-h" || a == "--help") { help_filter(); exit(0); }
             if (a == "-V" || a == "--version") { puts("Polypolish-filter v0.6.1"); exit(0); }
-            return filter_option(a, g);
+            return filter_option(a, g) || gpu_count_option(a, g);
         });
         if (g.in1.empty() || g.in2.empty() || g.out1.empty() || g.out2.empty())
             usage_error("the following required arguments were not provided:\n  --in1 <IN1>\n  --in2 <IN2>\n  --out1 <OUT1>\n  --out2 <OUT2>");
         std::vector<pp_ctx*> ctxs = open_contexts(g);
-        if (!g.quiet) fprintf(stderr, "Starting Polypolish filter (H100 build %s)\n\n", pp_version());
-        const int rc = pp_filter_files(ctxs[0], g.in1.c_str(), g.in2.c_str(), g.out1.c_str(), g.out2.c_str(), g.orientation.c_str(), g.low, g.high,
-                                       g.quiet ? 0 : 1);
+        if (!g.quiet) fprintf(stderr, "Starting Polypolish filter (H100 build %s%s)\n\n", pp_version(), g.gpus > 1 ? (", " + std::to_string(g.gpus) + " GPUs").c_str() : "");
+        const int rc = pp_filter_files_multi(ctxs.data(), g.gpus, g.in1.c_str(), g.in2.c_str(), g.out1.c_str(), g.out2.c_str(), g.orientation.c_str(),
+                                             g.low, g.high, g.quiet ? 0 : 1);
         finish(ctxs, rc, nullptr, 0, g.quiet);
     }
     if (cmd == "filter-polish") {
@@ -290,15 +299,15 @@ int main(int argc, char** argv) {
                 puts("Options: those of `filter` (--out1 / --out2 optional: written only when given) and of `polish` (except --debug)");
                 exit(0);
             }
-            return filter_option(a, g) || polish_option(a, g);
+            return filter_option(a, g) || polish_option(a, g) || gpu_count_option(a, g);
         });
         if (g.in1.empty() || g.in2.empty() || g.pos.size() != 1)
             usage_error("the following required arguments were not provided:\n  --in1 <IN1>\n  --in2 <IN2>\n  <ASSEMBLY>");
         std::vector<pp_ctx*> ctxs = open_contexts(g);
-        if (!g.quiet) fprintf(stderr, "Starting Polypolish filter + polish (H100 build %s)\n\n", pp_version());
-        const int rc = pp_filter_polish_files(ctxs[0], g.pos[0].c_str(), g.in1.c_str(), g.in2.c_str(), g.out1.empty() ? nullptr : g.out1.c_str(),
-                                              g.out2.empty() ? nullptr : g.out2.c_str(), g.orientation.c_str(), g.low, g.high, &g.prm, &out, &n,
-                                              g.quiet ? 0 : 1);
+        if (!g.quiet) fprintf(stderr, "Starting Polypolish filter + polish (H100 build %s%s)\n\n", pp_version(), g.gpus > 1 ? (", " + std::to_string(g.gpus) + " GPUs").c_str() : "");
+        const int rc = pp_filter_polish_files_multi(ctxs.data(), g.gpus, g.pos[0].c_str(), g.in1.c_str(), g.in2.c_str(),
+                                                    g.out1.empty() ? nullptr : g.out1.c_str(), g.out2.empty() ? nullptr : g.out2.c_str(),
+                                                    g.orientation.c_str(), g.low, g.high, &g.prm, &out, &n, g.quiet ? 0 : 1);
         finish(ctxs, rc, out, n, g.quiet);
     }
     usage_error("unrecognized subcommand '" + cmd + "'");

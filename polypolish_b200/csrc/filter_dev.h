@@ -15,6 +15,46 @@ struct Mate {
     uint32_t n;
 };
 
+struct FilterDev {
+    Mate m[2];
+    uint32_t n_names;
+    uint32_t* ins;             // [n_names] insert size of the unique pair
+    uint8_t* ori;              // [n_names] orientation 0..3 of the unique pair, 255 = not a unique pair
+    unsigned long long* pairs; // [4]
+    // radix select state for two ranks
+    uint32_t* hist;            // [2][256]
+    uint32_t* sel_prefix;      // [2]
+    unsigned long long* sel_rank; // [2] remaining rank (1-based) inside the current prefix
+    unsigned long long* n_pass;   // [2] passing records per mate
+};
+
+// One digit of the radix select: the bucket of `hist` (256 counts) that holds the rank-th value; `rank` becomes the rank inside it.
+#ifdef __CUDACC__
+__host__ __device__
+#endif
+inline uint32_t filter_pick_digit(const uint32_t* hist, unsigned long long& rank) {
+    uint32_t d = 0;
+    for (; d < 256; ++d) {
+        const uint32_t c = hist[d];
+        if (rank <= c) break;
+        rank -= c;
+    }
+    return d > 255 ? 255 : d;
+}
+
+// The filter proper in phases (filter_kernels.cu), so that one context (pp_filter_core) and several (tok_kernels.cu, each holding
+// the records of the read names it owns) run the same kernels and the same rules:
+//   filter_begin        per-name lists and unique pairs (k_f_build, k_f_pairs); f->pairs is ready when the stream is
+//   filter_orientation  the chosen orientation from the four pair counts, or the reference's error (filter.rs:168-177, 221-246)
+//   filter_ranks        the two nearest ranks (filter.rs:249-259) and whether each exists (sorted_list.get(rank - 1).unwrap_or(0))
+//   filter_hist         one digit of the radix select under the given prefixes: the 2 x 256 counts, on the host
+//   filter_pass         alignment_pass_qc for every record (k_f_pass); f->m[k].pass and f->n_pass are ready when the stream is
+int filter_begin(pp_ctx* ctx, const Mate in[2], uint32_t n_names, FilterDev* f, uint32_t* launches);
+int filter_orientation(pp_ctx* ctx, const pp_filter_params* prm, const unsigned long long pairs[4], int* chosen, unsigned long long* n_sizes);
+void filter_ranks(const pp_filter_params* prm, unsigned long long n_sizes, unsigned long long sel_rank[2], bool in_range[2]);
+int filter_hist(pp_ctx* ctx, const FilterDev& f, uint32_t chosen, int shift, uint32_t done_mask, const uint32_t prefix[2], uint32_t hist[512],
+                uint32_t* launches);
+void filter_pass(pp_ctx* ctx, const FilterDev& f, uint32_t low, uint32_t high, uint32_t chosen, uint32_t* launches);
 
 int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, pp_filter_result* res, const uint8_t* d_pass[2],
                    uint64_t n_pass_mate[2]);

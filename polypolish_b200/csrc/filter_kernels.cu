@@ -32,19 +32,6 @@ cudaEvent_t pp_ctx_event(pp_ctx* ctx, int i);
 
 #include "filter_dev.h"
 
-struct FilterDev {
-    Mate m[2];
-    uint32_t n_names;
-    uint32_t* ins;             // [n_names] insert size of the unique pair
-    uint8_t* ori;              // [n_names] orientation 0..3 of the unique pair, 255 = not a unique pair
-    unsigned long long* pairs; // [4]
-    // radix select state for two ranks
-    uint32_t* hist;            // [2][256]
-    uint32_t* sel_prefix;      // [2]
-    unsigned long long* sel_rank; // [2] remaining rank (1-based) inside the current prefix
-    unsigned long long* n_pass;   // [2] passing records per mate
-};
-
 // filter.rs:189-218.  Orientation codes: 0 fr, 1 rf, 2 ff, 3 rr.
 __device__ __forceinline__ void orient_insert(uint32_t s1, uint32_t e1, bool rev1, uint32_t s2, uint32_t e2, bool rev2,
                                               uint32_t& orientation, uint32_t& insert) {
@@ -116,14 +103,7 @@ __global__ void k_f_pick(FilterDev f, int shift) {      // one warp; lanes 0 and
     const int r = threadIdx.x;
     if (r < 2) {
         unsigned long long rank = f.sel_rank[r];
-        uint32_t d = 0;
-        for (; d < 256; ++d) {
-            const uint32_t c = f.hist[r * 256 + d];
-            if (rank <= c) break;
-            rank -= c;
-        }
-        if (d > 255) d = 255;
-        f.sel_prefix[r] |= d << shift;
+        f.sel_prefix[r] |= filter_pick_digit(f.hist + r * 256, rank) << shift;
         f.sel_rank[r] = rank;
     }
     __syncthreads();
@@ -165,14 +145,12 @@ static unsigned long long nearest_rank(double percentile, unsigned long long n) 
     return rank < 1 ? 1 : rank;
 }
 
-// The filter proper on device-resident mate arrays (in[k].name_id / contig / ref_start / ref_end / flags and n set by the
-// caller; host arrays are uploaded by pp_filter, the device SAM path of tok_kernels.cu builds them in place).
-// res->pass1/pass2 may be null: the flags then stay on the device only (d_pass[k], inside the context's scratch buffer,
-// valid until the next call that uses it).  n_pass_mate[k] = passing records of mate k.
-int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, pp_filter_result* res, const uint8_t* d_pass[2],
-                   uint64_t n_pass_mate[2]) {
+static unsigned grid_for(pp_ctx* ctx, size_t n) {
+    return (unsigned)std::min<size_t>(std::max<size_t>((n + 255) / 256, 1), (size_t)pp_ctx_sm_count(ctx) * 8);
+}
+
+int filter_begin(pp_ctx* ctx, const Mate in[2], uint32_t nn, FilterDev* out, uint32_t* launches) {
     cudaStream_t s = pp_ctx_stream(ctx);
-    const uint32_t nn = (uint32_t)prm->n_names;
     size_t off = 0;
     auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~size_t(255); return o; };
     size_t o_cnt[2], o_head[2], o_next[2], o_pass[2];
@@ -187,7 +165,7 @@ int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, p
     uint8_t* base = (uint8_t*)pp_ctx_scratch(ctx, off + 256);
     if (!base) return pp_ctx_fail(ctx, PP_ERR_NOMEM, "pp_filter: device allocation failed");
 
-    FilterDev f;
+    FilterDev& f = *out;
     for (int k = 0; k < 2; ++k) {
         f.m[k] = in[k];
         f.m[k].cnt = (uint32_t*)(base + o_cnt[k]); f.m[k].head = (uint32_t*)(base + o_head[k]);
@@ -201,18 +179,15 @@ int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, p
     CKF(cudaMemsetAsync(base + zero_begin, 0, zero_end - zero_begin, s));
     CKF(cudaMemsetAsync(base + zero_end, 0xFF, ff_end - zero_end, s));
     CKF(cudaEventRecord(pp_ctx_event(ctx, 1), s));
-
-    auto grid = [&](size_t n) { return (unsigned)std::min<size_t>(std::max<size_t>((n + 255) / 256, 1), (size_t)pp_ctx_sm_count(ctx) * 8); };
-    uint32_t launches = 0;
     for (int k = 0; k < 2; ++k)
-        if (in[k].n) { k_f_build<<<grid(in[k].n), 256, 0, s>>>(f, k); launches++; }
-    k_f_pairs<<<grid(nn), 256, 0, s>>>(f);
-    launches++;
-    unsigned long long pairs[4];
-    CKF(cudaMemcpyAsync(pairs, f.pairs, 32, cudaMemcpyDeviceToHost, s));
-    CKF(cudaStreamSynchronize(s));
-    CKF(cudaGetLastError());
-    for (int i = 0; i < 4; ++i) res->pairs[i] = pairs[i];
+        if (in[k].n) { k_f_build<<<grid_for(ctx, in[k].n), 256, 0, s>>>(f, k); ++*launches; }
+    k_f_pairs<<<grid_for(ctx, nn), 256, 0, s>>>(f);
+    ++*launches;
+    return PP_OK;
+}
+
+int filter_orientation(pp_ctx* ctx, const pp_filter_params* prm, const unsigned long long pairs[4], int* chosen_out,
+                       unsigned long long* n_sizes) {
     // filter.rs:168-177, 221-246
     if (pairs[0] + pairs[1] + pairs[2] + pairs[3] == 0)
         return pp_ctx_fail(ctx, PP_ERR_INPUT, "no one-alignment-per-read pairs available to determine orientation and insert size thresholds");
@@ -223,19 +198,70 @@ int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, p
         for (int i = 0; i < 4; ++i) if (pairs[i] == mx) { n_max++; chosen = i; }
         if (n_max != 1) return pp_ctx_fail(ctx, PP_ERR_INPUT, "could not automatically determine read pair orientation");
     }
-    const unsigned long long n_sizes = (chosen >= 0 && chosen < 4) ? pairs[chosen] : 0;
-    if (n_sizes == 0) return pp_ctx_fail(ctx, PP_ERR_INPUT, "no read pairs available to determine insert size thresholds");
+    *n_sizes = (chosen >= 0 && chosen < 4) ? pairs[chosen] : 0;
+    if (*n_sizes == 0) return pp_ctx_fail(ctx, PP_ERR_INPUT, "no read pairs available to determine insert size thresholds");
+    *chosen_out = chosen;
+    return PP_OK;
+}
+
+void filter_ranks(const pp_filter_params* prm, unsigned long long n_sizes, unsigned long long sel_rank[2], bool in_range[2]) {
+    const unsigned long long ranks[2] = {nearest_rank(prm->low_pct, n_sizes), nearest_rank(prm->high_pct, n_sizes)};
+    for (int r = 0; r < 2; ++r) {
+        in_range[r] = ranks[r] <= n_sizes;                               // sorted_list.get(rank-1).unwrap_or(0)
+        sel_rank[r] = in_range[r] ? ranks[r] : 1;
+    }
+}
+
+int filter_hist(pp_ctx* ctx, const FilterDev& f, uint32_t chosen, int shift, uint32_t done_mask, const uint32_t prefix[2], uint32_t hist[512],
+                uint32_t* launches) {
+    cudaStream_t s = pp_ctx_stream(ctx);
+    CKF(cudaMemcpyAsync(f.sel_prefix, prefix, 8, cudaMemcpyHostToDevice, s));
+    CKF(cudaMemsetAsync(f.hist, 0, 512 * 4, s));
+    k_f_hist<<<grid_for(ctx, f.n_names), 256, 0, s>>>(f, chosen, shift, done_mask);
+    ++*launches;
+    CKF(cudaMemcpyAsync(hist, f.hist, 512 * 4, cudaMemcpyDeviceToHost, s));
+    CKF(cudaStreamSynchronize(s));
+    CKF(cudaGetLastError());
+    return PP_OK;
+}
+
+void filter_pass(pp_ctx* ctx, const FilterDev& f, uint32_t low, uint32_t high, uint32_t chosen, uint32_t* launches) {
+    for (int k = 0; k < 2; ++k)
+        if (f.m[k].n) { k_f_pass<<<grid_for(ctx, f.m[k].n), 256, 0, pp_ctx_stream(ctx)>>>(f, k, low, high, chosen); ++*launches; }
+}
+
+// The filter proper on device-resident mate arrays (in[k].name_id / contig / ref_start / ref_end / flags and n set by the
+// caller; host arrays are uploaded by pp_filter, the device SAM path of tok_kernels.cu builds them in place).
+// res->pass1/pass2 may be null: the flags then stay on the device only (d_pass[k], inside the context's scratch buffer,
+// valid until the next call that uses it).  n_pass_mate[k] = passing records of mate k.
+int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, pp_filter_result* res, const uint8_t* d_pass[2],
+                   uint64_t n_pass_mate[2]) {
+    cudaStream_t s = pp_ctx_stream(ctx);
+    const uint32_t nn = (uint32_t)prm->n_names;
+    FilterDev f;
+    uint32_t launches = 0;
+    int rc = filter_begin(ctx, in, nn, &f, &launches);
+    if (rc != PP_OK) return rc;
+    unsigned long long pairs[4];
+    CKF(cudaMemcpyAsync(pairs, f.pairs, 32, cudaMemcpyDeviceToHost, s));
+    CKF(cudaStreamSynchronize(s));
+    CKF(cudaGetLastError());
+    for (int i = 0; i < 4; ++i) res->pairs[i] = pairs[i];
+    int chosen = 0;
+    unsigned long long n_sizes = 0;
+    rc = filter_orientation(ctx, prm, pairs, &chosen, &n_sizes);
+    if (rc != PP_OK) return rc;
     res->orientation = chosen;
 
     // exact nearest-rank percentiles by radix select (two ranks at once)
-    unsigned long long ranks[2] = {nearest_rank(prm->low_pct, n_sizes), nearest_rank(prm->high_pct, n_sizes)};
     uint32_t thr[2] = {0, 0};
-    bool in_range[2] = {ranks[0] <= n_sizes, ranks[1] <= n_sizes};     // sorted_list.get(rank-1).unwrap_or(0)
-    unsigned long long sel_rank[2] = {in_range[0] ? ranks[0] : 1, in_range[1] ? ranks[1] : 1};
+    bool in_range[2];
+    unsigned long long sel_rank[2];
+    filter_ranks(prm, n_sizes, sel_rank, in_range);
     CKF(cudaMemcpyAsync(f.sel_rank, sel_rank, 16, cudaMemcpyHostToDevice, s));
     uint32_t done_mask = 0;
     for (int shift = 24; shift >= 0; shift -= 8) {
-        k_f_hist<<<grid(nn), 256, 0, s>>>(f, (uint32_t)chosen, shift, done_mask);
+        k_f_hist<<<grid_for(ctx, nn), 256, 0, s>>>(f, (uint32_t)chosen, shift, done_mask);
         k_f_pick<<<1, 32, 0, s>>>(f, shift);
         launches += 2;
         done_mask |= 255u << shift;
@@ -246,8 +272,7 @@ int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, p
     res->low = in_range[0] ? thr[0] : 0;
     res->high = in_range[1] ? thr[1] : 0;
 
-    for (int k = 0; k < 2; ++k)
-        if (in[k].n) { k_f_pass<<<grid(in[k].n), 256, 0, s>>>(f, k, res->low, res->high, (uint32_t)chosen); launches++; }
+    filter_pass(ctx, f, res->low, res->high, (uint32_t)chosen, &launches);
     CKF(cudaEventRecord(pp_ctx_event(ctx, 2), s));
     if (in[0].n && res->pass1) CKF(cudaMemcpyAsync(res->pass1, f.m[0].pass, in[0].n, cudaMemcpyDeviceToHost, s));
     if (in[1].n && res->pass2) CKF(cudaMemcpyAsync(res->pass2, f.m[1].pass, in[1].n, cudaMemcpyDeviceToHost, s));

@@ -132,6 +132,26 @@ int pp::check_filter_args(pp_ctx* ctx, const char* in1, const char* in2, const c
     return PP_OK;
 }
 
+// get_insert_size_thresholds' log (filter.rs:168-186)
+static void log_thresholds(const char* orientation, const pp_filter_params* prm, const pp_filter_result* res) {
+    static const char* nm[4] = {"fr", "rf", "ff", "rr"};
+    for (int i = 0; i < 4; ++i) fprintf(stderr, "%s: %s pairs\n", nm[i], pp::thousands(res->pairs[i]).c_str());
+    fprintf(stderr, "\n%s correct orientation: %s\n\n", prm->orientation < 0 ? "Automatically determined" : "User-specified",
+            res->orientation < 4 ? nm[res->orientation] : orientation);
+    fprintf(stderr, "Low threshold:  %u\nHigh threshold: %u\n\n", res->low, res->high);
+}
+
+void pp_filter_log(const char* in1, const char* in2, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res,
+                   const pp_filter_file_stats* fs) {
+    const char* ins[2] = {in1, in2};
+    for (int k = 0; k < 2; ++k) fprintf(stderr, "%s: %s alignments\n", ins[k], pp::thousands(fs->alignments[k]).c_str());
+    log_thresholds(orientation, prm, res);
+    for (int k = 0; k < 2; ++k)
+        fprintf(stderr, "Filtering %s:\n  %s pass\n  %s fail\n\n", ins[k], pp::thousands(fs->pass[k]).c_str(), pp::thousands(fs->fail[k]).c_str());
+    fprintf(stderr, "Alignments before filtering: %s\nAlignments after filtering:  %s\n\n", pp::thousands(fs->alignments[0] + fs->alignments[1]).c_str(),
+            pp::thousands(fs->pass[0] + fs->pass[1]).c_str());
+}
+
 extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, const char* out1, const char* out2,
                                const char* orientation, double low, double high, int verbose) {
     if (!ctx) return PP_ERR_ARG;
@@ -140,15 +160,7 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
     if (int rc = pp::check_filter_args(ctx, in1, in2, out1, out2, orientation, low, high, &prm); rc != PP_OK) return rc;
     pp_filter_result res;
     memset(&res, 0, sizeof res);
-    const char* ins[2] = {in1, in2};
     const char* outs[2] = {out1, out2};
-    const char* nm[4] = {"fr", "rf", "ff", "rr"};
-    auto log_thresholds = [&]() {
-        for (int i = 0; i < 4; ++i) fprintf(stderr, "%s: %s pairs\n", nm[i], pp::thousands(res.pairs[i]).c_str());
-        fprintf(stderr, "\n%s correct orientation: %s\n\n", prm.orientation < 0 ? "Automatically determined" : "User-specified",
-                res.orientation < 4 ? nm[res.orientation] : orientation);
-        fprintf(stderr, "Low threshold:  %u\nHigh threshold: %u\n\n", res.low, res.high);
-    };
 
     // Fast path: the SAM text never leaves the device between parse and write (tok_kernels.cu).  PP_TOK_HOST = something the
     // device path leaves to the host code below (malformed line, empty file, ...), which words the reference's messages.
@@ -157,12 +169,7 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
         int rc = pp_filter_files_device(ctx, in1, in2, out1, out2, &prm, &res, &fs, nullptr);
         if (rc == PP_OK) {
             if (verbose) {
-                for (int k = 0; k < 2; ++k) fprintf(stderr, "%s: %s alignments\n", ins[k], pp::thousands(fs.alignments[k]).c_str());
-                log_thresholds();
-                for (int k = 0; k < 2; ++k)
-                    fprintf(stderr, "Filtering %s:\n  %s pass\n  %s fail\n\n", ins[k], pp::thousands(fs.pass[k]).c_str(), pp::thousands(fs.fail[k]).c_str());
-                fprintf(stderr, "Alignments before filtering: %s\nAlignments after filtering:  %s\n\n", pp::thousands(fs.alignments[0] + fs.alignments[1]).c_str(),
-                        pp::thousands(fs.pass[0] + fs.pass[1]).c_str());
+                pp_filter_log(in1, in2, orientation, &prm, &res, &fs);
                 fprintf(stderr, "device text path: %.3f ms (SAM to HBM %.3f ms, filtered SAM to files %.3f ms), %u kernels; filter kernels %.3f ms\n", fs.total_ms,
                         fs.h2d_ms, fs.d2h_ms, fs.launches, res.timing.total_ms);
                 fprintf(stderr, "  phases (wall ms): upload+index+parse %.1f, intern+verify+emit %.1f, filter %.1f, output offsets %.1f, output bytes %.1f, download+write %.1f\n",
@@ -198,7 +205,7 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
     res.pass2 = pass2.data();
     int rc = pp_filter(ctx, &fm[0], &fm[1], &prm, &res);
     if (rc != PP_OK) return rc;
-    if (verbose) log_thresholds();
+    if (verbose) log_thresholds(orientation, &prm, &res);
     uint64_t before = fm[0].n + fm[1].n, after = 0;
     const uint8_t* passes[2] = {pass1.data(), pass2.data()};
     for (int k = 0; k < 2; ++k) {
@@ -213,4 +220,37 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
         fprintf(stderr, "device path: %.3f ms, %u kernels\n", res.timing.total_ms, res.timing.launches);
     }
     return PP_OK;
+}
+
+// `polypolish filter` over several GPUs: GPU g filters byte range g of both files (pp_sam_split_ranges), the records meet on the GPU
+// that owns their read name, the thresholds are reduced across GPUs (tok_kernels.cu).  Whatever that path does not settle - the
+// host parser asked for, an input that is not a regular file, PP_TOK_HOST - is the one-context call's on ctxs[0].
+extern "C" int pp_filter_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                                     const char* orientation, double low, double high, int verbose) {
+    if (!ctxs || n_ctx < 1 || !ctxs[0]) return PP_ERR_ARG;
+    pp_ctx* ctx = ctxs[0];
+    for (int g = 1; g < n_ctx; ++g)
+        if (!ctxs[g]) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_files_multi: null context");
+    if (n_ctx == 1 || pp_get_parser(ctx) != 0) return pp_filter_files(ctx, in1, in2, out1, out2, orientation, low, high, verbose);
+    if (!in1 || !in2 || !out1 || !out2 || !orientation) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_files: null argument");
+    pp_filter_params prm;
+    if (int rc = pp::check_filter_args(ctx, in1, in2, out1, out2, orientation, low, high, &prm); rc != PP_OK) return rc;
+    std::vector<uint64_t> cuts[2] = {std::vector<uint64_t>((size_t)n_ctx + 1), std::vector<uint64_t>((size_t)n_ctx + 1)};
+    int rc = PP_TOK_HOST;
+    if (pp_sam_split_ranges(in1, n_ctx, cuts[0].data()) == PP_OK && pp_sam_split_ranges(in2, n_ctx, cuts[1].data()) == PP_OK) {
+        const uint64_t* c[2] = {cuts[0].data(), cuts[1].data()};
+        pp_filter_result res;
+        memset(&res, 0, sizeof res);
+        pp_filter_file_stats fs;
+        rc = pp_filter_files_device_multi(ctxs, n_ctx, in1, in2, out1, out2, &prm, c, &res, &fs, nullptr);
+        if (rc == PP_OK && verbose) {
+            pp_filter_log(in1, in2, orientation, &prm, &res, &fs);
+            fprintf(stderr, "device text path over %d GPUs: %.3f ms (SAM to HBM %.3f ms on the slowest GPU, filtered SAM to files %.3f ms), %u kernels\n", n_ctx,
+                    fs.total_ms, fs.h2d_ms, fs.d2h_ms, fs.launches);
+            fprintf(stderr, "  phases (wall ms): upload+index+parse+intern %.1f, records to their name's GPU %.1f, filter %.1f\n", fs.phase_ms[0],
+                    fs.phase_ms[1], fs.phase_ms[2]);
+        }
+    }
+    if (rc != PP_TOK_HOST) return rc;
+    return pp_filter_files(ctx, in1, in2, out1, out2, orientation, low, high, verbose);
 }

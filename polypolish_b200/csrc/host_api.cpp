@@ -222,33 +222,6 @@ struct FusedFilter {
     const char *out1, *out2;             // filtered SAM files, or null: not written
 };
 
-// filter (filter.rs:26-37) and the load of polish in one pass over the text: both files go to HBM once, the filter's verdict
-// becomes the ZP flag of the tokenised records (what ZP:Z:fail does after a round trip through two files).
-static int load_fused(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const char* const* sams, const FusedFilter& ff,
-                      int careful, Load& ld) {
-    pp_filter_result fres;
-    pp_filter_file_stats fs;
-    memset(&fres, 0, sizeof fres);
-    pp_fused_polish fuse;
-    memset(&fuse, 0, sizeof fuse);
-    fuse.fasta = fa; fuse.careful = careful;
-    int rc = pp_filter_files_device(ctx, sams[0], sams[1], ff.out1, ff.out2, &ff.prm, &fres, &fs, &fuse);
-    if (rc == PP_OK && fuse.rc == PP_TOK_HOST) rc = PP_TOK_HOST;
-    if (rc != PP_OK) return rc;
-    static const char* nm[4] = {"fr", "rf", "ff", "rr"};
-    char tmp[512];
-    for (int k = 0; k < 2; ++k) {
-        snprintf(tmp, sizeof tmp, "%s: %s alignments, %s pass the insert-size filter, %s fail\n", sams[k], pp::thousands(fs.alignments[k]).c_str(),
-                 pp::thousands(fs.pass[k]).c_str(), pp::thousands(fs.fail[k]).c_str());
-        ld.log += tmp;
-    }
-    snprintf(tmp, sizeof tmp, "orientation %s, insert size thresholds %u - %u\n", fres.orientation < 4 ? nm[fres.orientation] : ff.orientation, fres.low, fres.high);
-    ld.log += tmp;
-    ld.alns.n_aln = fuse.n_aln;
-    one_job(ld, ctx, contigs, true);
-    return PP_OK;
-}
-
 // Several GPUs, no host in the middle: the host only decides which contig goes where (longest contig first onto the lightest
 // shard, owner[c]) and where to cut the files (cuts[f][s], split_ranges); the text, the records and the shards never pass through
 // host memory as arrays.  Each job keeps its own contigs.  PP_TOK_HOST: a file cannot be cut.
@@ -286,6 +259,8 @@ static int plan_device_shards(pp_ctx* const* ctxs, uint32_t n, const pp_contigs&
         if (!split_ranges(sams[i], (int)n, cuts[(size_t)i])) return PP_TOK_HOST;
     return PP_OK;
 }
+
+static int exchange(const std::vector<uint32_t>& owner, uint32_t n_contigs, Load& ld);
 
 // SAM files -> resident datasets through the device tokeniser (tok_kernels.cu), on the contexts of ld.jobs: job s reads bytes
 // [cuts[f][s], cuts[f][s + 1]) of every file f, the whole files when there is one job.  Bases are packed 4 bits wide, 8 when a read
@@ -338,6 +313,12 @@ static int tokenise(const pp_fasta* fa, const char* const* sams, int n_sams, int
     }
     ld.alns.n_aln = n_aln;
     if (n == 1) return pp_tok_finish(ld.jobs[0].ctx);
+    return exchange(owner, n_contigs, ld);
+}
+
+// Several jobs with tokenised ranges: every read group goes to the GPUs that own its contigs (pp_tok_exchange_finish).
+static int exchange(const std::vector<uint32_t>& owner, uint32_t n_contigs, Load& ld) {
+    const uint32_t n = (uint32_t)ld.jobs.size();
     std::vector<pp_ctx*> ctxs(n);
     std::vector<const uint32_t*> lo(n);
     std::vector<pp_contigs> sc(n);
@@ -372,6 +353,50 @@ static int load_device(pp_ctx* const* ctxs, uint32_t n, const pp_fasta* fa, cons
     const int rc = tokenise(fa, sams, n_sams, careful, cuts, owner, contigs.n_contigs, ld);
     ld.jobs[0].alns = ld.alns;
     return rc;
+}
+
+// filter (filter.rs:26-37) and the load of polish in one pass over the text: both files go to HBM once, the filter's verdict
+// becomes the ZP flag of the tokenised records (what ZP:Z:fail does after a round trip through two files).  Several GPUs each filter
+// and tokenise byte range g of both files (the read names meet on their owner GPU for the filter), then exchange read groups by
+// contig exactly like `polish` over several GPUs.
+static int load_fused(pp_ctx* const* ctxs, uint32_t n, const pp_fasta* fa, const pp_contigs& contigs, const char* const* sams, const FusedFilter& ff,
+                      int careful, Load& ld) {
+    pp_ctx* ctx = ctxs[0];
+    pp_filter_result fres;
+    pp_filter_file_stats fs;
+    memset(&fres, 0, sizeof fres);
+    pp_fused_polish fuse;
+    memset(&fuse, 0, sizeof fuse);
+    fuse.fasta = fa; fuse.careful = careful;
+    std::vector<uint32_t> owner;
+    std::vector<std::vector<uint64_t>> cuts;
+    int rc;
+    if (n == 1) {
+        rc = pp_filter_files_device(ctx, sams[0], sams[1], ff.out1, ff.out2, &ff.prm, &fres, &fs, &fuse);
+    } else {
+        rc = plan_device_shards(ctxs, n, contigs, sams, 2, ld, owner, cuts);
+        const uint64_t* c[2] = {cuts.size() == 2 ? cuts[0].data() : nullptr, cuts.size() == 2 ? cuts[1].data() : nullptr};
+        if (rc == PP_OK) rc = pp_filter_files_device_multi(ctxs, (int)n, sams[0], sams[1], ff.out1, ff.out2, &ff.prm, c, &fres, &fs, &fuse);
+    }
+    if (rc == PP_OK && fuse.rc == PP_TOK_HOST) rc = PP_TOK_HOST;
+    if (rc != PP_OK) return rc;
+    static const char* nm[4] = {"fr", "rf", "ff", "rr"};
+    char tmp[512];
+    for (int k = 0; k < 2; ++k) {
+        snprintf(tmp, sizeof tmp, "%s: %s alignments, %s pass the insert-size filter, %s fail\n", sams[k], pp::thousands(fs.alignments[k]).c_str(),
+                 pp::thousands(fs.pass[k]).c_str(), pp::thousands(fs.fail[k]).c_str());
+        ld.log += tmp;
+    }
+    snprintf(tmp, sizeof tmp, "orientation %s, insert size thresholds %u - %u\n", fres.orientation < 4 ? nm[fres.orientation] : ff.orientation, fres.low, fres.high);
+    ld.log += tmp;
+    ld.alns.n_aln = fuse.n_aln;
+    if (n == 1) {
+        one_job(ld, ctx, contigs, true);
+        return PP_OK;
+    }
+    snprintf(tmp, sizeof tmp, "filter over %u GPUs (records to the GPU of their read name, thresholds reduced across GPUs): %.3f ms\n", n, fs.total_ms);
+    ld.timing += tmp;
+    return exchange(owner, contigs.n_contigs, ld);
 }
 
 // The host packer (sam_pack.cpp): the text is parsed on the host, then split into n shards by pp_shards_build.  PP_OK or an error.
@@ -576,7 +601,7 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     Load ld;
     int rc = PP_TOK_HOST;
     if (device_parser && (ff || n_sams > 0)) {
-        rc = ff ? load_fused(ctx, fa.get(), contigs, sams, *ff, prm->careful, ld)
+        rc = ff ? load_fused(ctxs, n_shards, fa.get(), contigs, sams, *ff, prm->careful, ld)
                 : load_device(ctxs, n_shards, fa.get(), contigs, sams, n_sams, prm->careful, ld);
         if (rc == PP_OK) run_jobs(ld.jobs, prm);
         if (rc == PP_OK && data_error(ld.jobs)) rc = PP_TOK_HOST;
@@ -652,6 +677,28 @@ extern "C" int pp_filter_polish_files(pp_ctx* ctx, const char* assembly, const c
     if (!out1) unlink(t1.c_str());
     if (!out2) unlink(t2.c_str());
     return rc;
+}
+
+// The same over several GPUs of one box: every GPU filters and tokenises its byte range of both files, the read names meet on their
+// owner GPU for the filter, the read groups on their contigs' GPUs for the polish.  More than 32 contexts, and whatever that path does
+// not settle, are the one-context call's on ctxs[0].
+extern "C" int pp_filter_polish_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* assembly, const char* in1, const char* in2, const char* out1,
+                                            const char* out2, const char* orientation, double low, double high, const pp_polish_params* prm,
+                                            char** out_fasta, uint64_t* out_len, int verbose) {
+    if (!ctxs || n_ctx < 1 || !ctxs[0]) return PP_ERR_ARG;
+    pp_ctx* ctx = ctxs[0];
+    for (int g = 1; g < n_ctx; ++g)
+        if (!ctxs[g]) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_polish_files_multi: null context");
+    if (n_ctx == 1 || n_ctx > 32)
+        return pp_filter_polish_files(ctx, assembly, in1, in2, out1, out2, orientation, low, high, prm, out_fasta, out_len, verbose);
+    if (!in1 || !in2 || !orientation) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_polish_files: null argument");
+    FusedFilter ff{{}, orientation, out1, out2};
+    int rc = pp::check_filter_args(ctx, in1, in2, out1, out2, orientation, low, high, &ff.prm);
+    if (rc != PP_OK) return rc;
+    const char* sams[2] = {in1, in2};
+    rc = polish_files_impl(ctxs, n_ctx, assembly, sams, 2, prm, nullptr, out_fasta, out_len, verbose, &ff);
+    if (rc != PP_TOK_HOST) return rc;
+    return pp_filter_polish_files(ctx, assembly, in1, in2, out1, out2, orientation, low, high, prm, out_fasta, out_len, verbose);
 }
 
 extern "C" int pp_polish_files(pp_ctx* ctx, const char* assembly, const char* const* sams, int n_sams,

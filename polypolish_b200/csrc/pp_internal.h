@@ -128,3 +128,13 @@ struct pp_fused_polish {
 };
 int pp_filter_files_device(pp_ctx* ctx, const char* in1, const char* in2, const char* out1, const char* out2, const pp_filter_params* prm,
                            pp_filter_result* res, pp_filter_file_stats* fs, pp_fused_polish* fuse);
+// The same over several contexts: context g reads bytes [cuts[f][g], cuts[f][g + 1]) of file f (cut between read groups), and the
+// records meet on the context that owns their read name.  With `fuse` every context then tokenises its ranges for polish
+// (pp_tok_set_ranges) with the verdicts as ZP flags, ready for pp_tok_exchange_finish.  fs and fuse->stats are sums over the
+// contexts; errors are reported on ctxs[0].  PP_OK, PP_TOK_HOST (the one-context call must do it) or an error.
+int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                                 const pp_filter_params* prm, const uint64_t* const cuts[2], pp_filter_result* res, pp_filter_file_stats* fs,
+                                 pp_fused_polish* fuse);
+// the filter's log on stderr (filter.rs:26-37 and the functions it calls), shared by the one-context and the multi-context calls
+void pp_filter_log(const char* in1, const char* in2, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res,
+                   const pp_filter_file_stats* fs);

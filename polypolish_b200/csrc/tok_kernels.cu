@@ -1369,8 +1369,9 @@ __global__ void __launch_bounds__(256) k_ftok_copy(FileDev f, const uint8_t* __r
 // Streams n device bytes into fd (the mirror image of upload_file): each thread copies its slices into its pinned slots and
 // from there into the file.  `map` is the file mapped MAP_SHARED (page faults of different threads proceed in parallel,
 // whereas write()s to one file serialise on its inode lock: 3 GB/s on tmpfs whatever the thread count); when the mapping
-// could not be made, pwrite() is used.  PP_OK / PP_ERR_IO / PP_ERR_CUDA.
-static int download_file(int device, TokState* T, const uint8_t* src, int fd, uint8_t* map, uint64_t n, int* cuda_err) {
+// could not be made, pwrite() is used.  The bytes land at [base, base + n) of the file (`map` maps the whole file).
+// PP_OK / PP_ERR_IO / PP_ERR_CUDA.
+static int download_file(int device, TokState* T, const uint8_t* src, int fd, uint8_t* map, uint64_t n, int* cuda_err, uint64_t base = 0) {
     const int R = T->readers;
     const uint64_t n_slices = (n + TK_SLOT - 1) / TK_SLOT;
     std::atomic<int> err{0}, cerr{0};
@@ -1381,10 +1382,10 @@ static int download_file(int device, TokState* T, const uint8_t* src, int fd, ui
         auto flush_prev = [&](int slot) -> bool {
             cudaError_t e = cudaEventSynchronize(T->rev[r][slot]);
             if (e != cudaSuccess) { cerr = (int)e; err = 2; return false; }
-            if (map) { memcpy(map + prev_o, T->pin[r][slot], (size_t)prev_len); return true; }
+            if (map) { memcpy(map + base + prev_o, T->pin[r][slot], (size_t)prev_len); return true; }
             uint64_t put = 0;
             while (put < prev_len) {
-                const ssize_t g = pwrite(fd, T->pin[r][slot] + put, (size_t)(prev_len - put), (off_t)(prev_o + put));
+                const ssize_t g = pwrite(fd, T->pin[r][slot] + put, (size_t)(prev_len - put), (off_t)(base + prev_o + put));
                 if (g <= 0) { err = 1; return false; }
                 put += (uint64_t)g;
             }
@@ -1489,11 +1490,13 @@ static int ftok_lines(pp_ctx* ctx, TokState* T, int which, const uint8_t* text, 
 
 struct TokFilterBufs {                 // device buffers of the filter text path, kept in the tokeniser state
     DevBuf lines[2], tmp[2], mate[2], table, out, status, passkeep;
+    DevBuf fx_refs, fx_stage, fx_rx, fx_owner, fx_home;   // pp_filter_files_multi: see there
 };
 
 static void free_filter_bufs(TokFilterBufs* b) {
     for (int k = 0; k < 2; ++k) { b->lines[k].release(); b->tmp[k].release(); b->mate[k].release(); }
     b->table.release(); b->out.release(); b->status.release(); b->passkeep.release();
+    b->fx_refs.release(); b->fx_stage.release(); b->fx_rx.release(); b->fx_owner.release(); b->fx_home.release();
     delete b;
 }
 
@@ -1706,6 +1709,679 @@ int pp_filter_files_device(pp_ctx* ctx, const char* in1, const char* in2, const 
             fuse->rc = rc;
             break;
         }
+    }
+    fs->total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+    return PP_OK;
+}
+
+// =====================================================================================================================
+// `polypolish filter` over several GPUs (pp_filter_files_multi).  GPU g reads byte range g of both files (cut between read groups,
+// so `filter-polish` can hand the same ranges to the polish tokeniser), indexes, parses and interns its lines as above.
+// A record's verdict (alignment_pass_qc, filter.rs:352-377) depends only on the set of alignments that share its read name, and
+// the insert-size statistics are sums over names, so the work partitions by read name:
+//   k_fx_refs / k_fx_ref_bytes  every GPU's distinct RNAME strings go to the host, which numbers them by string (exact, no hash
+//                               trust) and sends back a local -> global table (k_fx_scatter)
+//   k_fx_count                  per destination: records, distinct names, name bytes (destination = owner of the QNAME key)
+//   k_fx_names / k_fx_recs      compact records and each distinct name once (key + bytes) into per-destination staging, already
+//                               numbered for their place at the destination; peer copies move them
+//   k_fx_intern / k_fx_verify   the owner interns the names it received and confirms byte by byte that one key is one string
+//   k_fx_mates                  the owner's two Mate arrays; then filter_begin / filter_hist / filter_pass (filter_kernels.cu),
+//                               with the pair counts and the radix-select histograms summed on the host between the kernels
+//   k_fx_home                   the verdicts, copied back to the source GPU, land at (file, aligned index); each GPU then writes
+//                               its piece of each output file at its offset (k_ftok_outlen / k_ftok_copy / download_file)
+// =====================================================================================================================
+namespace {
+
+struct FxCount { unsigned long long names, bytes, recs[2]; };
+struct FxPlan { unsigned long long stage_name, stage_byte, stage_rec[2], name_base, byte_base; };
+struct FxName { unsigned long long key; uint32_t off, len; };             // a distinct QNAME: its key; its bytes at `off`
+struct FxRec { uint32_t name, contig, start, end, src, flags; };          // flags: bit 0 reverse strand, bit 1 second file
+struct FxRef { unsigned long long pos; uint32_t slot, len; };             // a distinct RNAME: file << 63 | text offset
+
+__device__ __forceinline__ uint32_t fx_owner(unsigned long long key, uint32_t n) {
+    key ^= key >> 31; key *= 0xBF58476D1CE4E5B9ull; key ^= key >> 29;
+    return (uint32_t)((key >> 32) % n);
+}
+
+__device__ __forceinline__ unsigned long long fx_who(int which, uint64_t i) { return ((unsigned long long)which << 40) | i; }
+
+__global__ void __launch_bounds__(TK_LINE_THREADS) k_fx_refs(FileDev f, int which, InternTable t, FxRef* out, unsigned long long* n_out, uint64_t cap) {
+    const uint64_t i = (uint64_t)blockIdx.x * TK_LINE_THREADS + threadIdx.x;
+    if (i >= f.n_lines) return;
+    const tok::FLineRec r = f.recs[i];
+    if (r.kind != tok::FK_ALIGNED) return;
+    const uint32_t sl = f.ref_slot[i];
+    if (t.rep[sl] != ((1ull << 62) | fx_who(which, i))) return;     // the first line of this RNAME
+    const unsigned long long j = atomicAdd(n_out, 1ull);
+    if (j < cap) out[j] = FxRef{((unsigned long long)which << 63) | (f.line_start[i] + r.ref_rel), sl, r.ref_len};
+}
+
+__global__ void __launch_bounds__(256) k_fx_ref_bytes(const FxRef* __restrict__ refs, uint64_t n, const unsigned long long* __restrict__ off,
+                                                      const uint8_t* __restrict__ t0, const uint8_t* __restrict__ t1, uint8_t* __restrict__ out) {
+    const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (j >= n) return;
+    const FxRef r = refs[j];
+    const uint8_t* t = (r.pos >> 63) ? t1 : t0;
+    const uint64_t p = r.pos & ~(1ull << 63);
+    for (uint32_t k = 0; k < r.len; ++k) out[off[j] + k] = t[p + k];
+}
+
+__global__ void __launch_bounds__(256) k_fx_scatter(const uint2* __restrict__ pairs, uint64_t n, uint32_t* __restrict__ slot_val) {
+    const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (j < n) slot_val[pairs[j].x] = pairs[j].y;
+}
+
+__global__ void __launch_bounds__(TK_LINE_THREADS) k_fx_count(FileDev f, int which, InternTable t, uint32_t n_dst, FxCount* cnt) {
+    const uint64_t i = (uint64_t)blockIdx.x * TK_LINE_THREADS + threadIdx.x;
+    if (i >= f.n_lines) return;
+    const tok::FLineRec r = f.recs[i];
+    if (r.kind != tok::FK_ALIGNED) return;
+    const uint32_t d = fx_owner(r.name_hash, n_dst);
+    atomicAdd(&cnt[d].recs[which], 1ull);
+    if (t.rep[f.name_slot[i]] == fx_who(which, i)) { atomicAdd(&cnt[d].names, 1ull); atomicAdd(&cnt[d].bytes, (unsigned long long)r.name_len); }
+}
+
+// Each distinct name once per source GPU: key and bytes to its owner's staging; slot_val[name slot] = its index at the owner.
+__global__ void __launch_bounds__(TK_LINE_THREADS) k_fx_names(FileDev f, int which, InternTable t, uint32_t n_dst, const FxPlan* __restrict__ plan,
+                                                              FxCount* at, FxName* __restrict__ names, uint8_t* __restrict__ bytes,
+                                                              uint32_t* __restrict__ slot_val) {
+    const uint64_t i = (uint64_t)blockIdx.x * TK_LINE_THREADS + threadIdx.x;
+    if (i >= f.n_lines) return;
+    const tok::FLineRec r = f.recs[i];
+    if (r.kind != tok::FK_ALIGNED || t.rep[f.name_slot[i]] != fx_who(which, i)) return;
+    const uint32_t d = fx_owner(r.name_hash, n_dst);
+    const FxPlan p = plan[d];
+    const unsigned long long j = atomicAdd(&at[d].names, 1ull), b = atomicAdd(&at[d].bytes, (unsigned long long)r.name_len);
+    names[p.stage_name + j] = FxName{r.name_hash, (uint32_t)(p.byte_base + b), r.name_len};
+    const uint64_t s = f.line_start[i];
+    for (uint32_t k = 0; k < r.name_len; ++k) bytes[p.stage_byte + b + k] = f.text[s + k];
+    slot_val[f.name_slot[i]] = (uint32_t)(p.name_base + j);
+}
+
+__global__ void __launch_bounds__(TK_LINE_THREADS) k_fx_recs(FileDev f, int which, uint32_t n_dst, const FxPlan* __restrict__ plan, FxCount* at,
+                                                             const uint32_t* __restrict__ slot_val, FxRec* __restrict__ recs) {
+    const uint64_t i = (uint64_t)blockIdx.x * TK_LINE_THREADS + threadIdx.x;
+    if (i >= f.n_lines) return;
+    const tok::FLineRec r = f.recs[i];
+    if (r.kind != tok::FK_ALIGNED) return;
+    const uint32_t d = fx_owner(r.name_hash, n_dst);
+    const unsigned long long j = atomicAdd(&at[d].recs[which], 1ull);
+    recs[plan[d].stage_rec[which] + j] = FxRec{slot_val[f.name_slot[i]], slot_val[f.ref_slot[i]], r.ref_start, r.ref_end, (uint32_t)f.s_al[i],
+                                               (uint32_t)r.rev | ((uint32_t)which << 1)};
+}
+
+__global__ void __launch_bounds__(256) k_fx_intern(const FxName* __restrict__ names, uint64_t n, InternTable t, uint32_t* __restrict__ id, FStatus* st) {
+    const uint64_t e = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (e < n) id[e] = intern(t, names[e].key, e, st);
+}
+
+// Every received name confirms, byte by byte, that the name that owns its slot is the same string.
+__global__ void __launch_bounds__(256) k_fx_verify(const FxName* __restrict__ names, uint64_t n, const uint8_t* __restrict__ bytes, InternTable t,
+                                                   const uint32_t* __restrict__ id, FStatus* st) {
+    const uint64_t e = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (e >= n) return;
+    const FxName a = names[e], b = names[t.rep[id[e]]];
+    bool same = a.len == b.len;
+    for (uint32_t k = 0; same && k < a.len; ++k) same = bytes[a.off + k] == bytes[b.off + k];
+    if (!same) st->collision = 1;
+}
+
+__global__ void __launch_bounds__(256) k_fx_mates(const FxRec* __restrict__ recs, uint64_t n, const uint32_t* __restrict__ id, MateOut m) {
+    const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (j >= n) return;
+    const FxRec r = recs[j];
+    m.name_id[j] = id[r.name];
+    m.contig[j] = r.contig;
+    m.ref_start[j] = r.start;
+    m.ref_end[j] = r.end;
+    m.flags[j] = (uint8_t)(r.flags & 1);
+}
+
+// The owners' verdicts, back in the staging order of this GPU, go to (file, aligned index).
+__global__ void __launch_bounds__(256) k_fx_home(const FxRec* __restrict__ recs, uint64_t n, const uint8_t* __restrict__ ret, uint8_t* __restrict__ pass0,
+                                                 uint8_t* __restrict__ pass1) {
+    const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (j >= n) return;
+    const FxRec r = recs[j];
+    ((r.flags & 2) ? pass1 : pass0)[r.src] = ret[j];
+}
+
+unsigned fx_blocks(uint64_t n, unsigned per) { return (unsigned)((n + per - 1) / per); }
+
+// One context of pp_filter_files_multi: its byte ranges as a source, the names it owns as an owner.
+struct FxSide {
+    pp_ctx* ctx = nullptr;
+    TokState* T = nullptr;
+    TokFilterBufs* B = nullptr;
+    FStatus* d_st = nullptr;
+    FileDev fd[2];
+    uint64_t n_al[2] = {0, 0};
+    InternTable tb{};
+    uint32_t* slot_val = nullptr;          // [table slots] after interning: global contig id (RNAME slots), index at the owner (QNAME slots)
+    // as a source
+    std::vector<FxRef> refs;
+    std::vector<uint64_t> ref_off;
+    std::vector<uint8_t> ref_bytes;
+    std::vector<uint2> ref_global;
+    std::vector<FxCount> cnt;              // [destination]
+    std::vector<FxPlan> plan;              // [destination]
+    uint64_t st_names = 0, st_bytes = 0, st_recs[2] = {0, 0};
+    FxCount* d_at = nullptr;
+    FxPlan* d_plan = nullptr;
+    FxName* s_names = nullptr;
+    uint8_t* s_bytes = nullptr;
+    FxRec* s_recs = nullptr;
+    uint8_t* ret = nullptr;                // [st_recs[0] + st_recs[1]] the owners' verdicts, staging order
+    uint8_t* pass[2] = {nullptr, nullptr}; // [n_al[k]] verdicts by aligned index
+    // as an owner
+    uint64_t rx_names = 0, rx_bytes = 0, rx_recs[2] = {0, 0};
+    FxName* r_names = nullptr;
+    uint8_t* r_bytes = nullptr;
+    FxRec* r_recs[2] = {nullptr, nullptr};
+    FilterDev f{};
+    unsigned long long pairs[4] = {0, 0, 0, 0}, np[2] = {0, 0};
+    uint32_t hist[512];
+    uint64_t out_n = 0;
+    uint32_t launches = 0;
+    uint64_t text_bytes[2] = {0, 0};
+    float h2d_ms = 0;
+    pp_tok_stats tst[2];
+};
+
+}  // namespace
+
+// fn(side, g) on every context, each on its own host thread; the first error (its message moved to ctxs[0]) before PP_TOK_HOST,
+// before PP_TOK_NEED8.
+template <class F>
+static int fx_all(std::vector<FxSide>& S, F&& fn) {
+    std::vector<int> rc(S.size(), PP_OK);
+    auto run = [&](size_t g) {
+        pp_ctx* ctx = S[g].ctx;
+        const cudaError_t e = cudaSetDevice(ctx->device);
+        rc[g] = e != cudaSuccess ? ctx->fail_cuda(e, "cudaSetDevice", __FILE__, __LINE__) : fn(S[g], (int)g);
+    };
+    std::vector<std::thread> th;
+    for (size_t g = 1; g < S.size(); ++g) th.emplace_back(run, g);
+    run(0);
+    for (auto& t : th) t.join();
+    for (size_t g = 0; g < S.size(); ++g)
+        if (rc[g] < 0) { if (g) S[0].ctx->err = S[g].ctx->err; return rc[g]; }
+    for (int want : {PP_TOK_HOST, PP_TOK_NEED8})
+        if (std::count(rc.begin(), rc.end(), want)) return want;
+    return PP_OK;
+}
+
+static int fx_copy(pp_ctx* ctx, pp_ctx* dctx, void* dst, const void* src, size_t bytes) {
+    if (!bytes) return PP_OK;
+    if (dctx->device == ctx->device) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    else CK(cudaMemcpyPeerAsync(dst, dctx->device, src, ctx->device, bytes, ctx->stream));
+    return PP_OK;
+}
+
+int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                                 const pp_filter_params* prm, const uint64_t* const cuts[2], pp_filter_result* res, pp_filter_file_stats* fs,
+                                 pp_fused_polish* fuse) {
+    const uint32_t n = (uint32_t)n_ctx;
+    pp_ctx* c0 = ctxs[0];
+    const char* ins[2] = {in1, in2};
+    const char* outs[2] = {out1, out2};
+    memset(fs, 0, sizeof *fs);
+    const auto t_begin = std::chrono::steady_clock::now();
+    std::vector<FxSide> S(n);
+    for (uint32_t g = 0; g < n; ++g) {
+        pp_ctx* ctx = ctxs[g];
+        S[g].ctx = ctx;
+        CK(cudaSetDevice(ctx->device));
+        int rc = tok_state(ctx, &S[g].T);
+        if (rc) { if (g) c0->err = ctx->err; return rc; }
+        if (!S[g].T->fbufs) S[g].T->fbufs = new TokFilterBufs();
+        S[g].B = S[g].T->fbufs;
+        for (uint32_t o = 0; o < n; ++o)                                    // NVLink between the GPUs where the box has it
+            if (ctxs[o]->device != ctx->device) {
+                int can = 0;
+                if (cudaDeviceCanAccessPeer(&can, ctx->device, ctxs[o]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[o]->device, 0);
+                cudaGetLastError();                                          // (already enabled is fine)
+            }
+    }
+
+    // ---- every GPU: its two ranges into HBM, lines, quick parse, local interning (as the one-GPU path)
+    int rc = fx_all(S, [&](FxSide& X, int g) -> int {
+        pp_ctx* ctx = X.ctx;
+        TokState* T = X.T;
+        TokFilterBufs& B = *X.B;
+        cudaStream_t s = ctx->stream;
+        CK(B.status.ensure(sizeof(FStatus)));
+        X.d_st = B.status.as<FStatus>();
+        FStatus h_st;
+        h_st.first_bad[0] = h_st.first_bad[1] = ~0ull; h_st.collision = 0; h_st.pad = 0;
+        CK(cudaMemcpyAsync(X.d_st, &h_st, sizeof h_st, cudaMemcpyHostToDevice, s));
+        CK(cudaStreamSynchronize(s));
+        T->range_off = {cuts[0][g], cuts[1][g]};
+        T->range_len = {cuts[0][g + 1] - cuts[0][g], cuts[1][g + 1] - cuts[1][g]};
+        uint32_t launches = 0;
+        for (int k = 0; k < 2; ++k) {
+            int r = prefetch_wait(ctx, T, ins[k], false, k);
+            if (r != PP_OK) return r;
+            const uint64_t nb = T->pf.n;
+            const uint8_t* text = T->text[T->pf.buf].as<uint8_t>();
+            const bool unterminated = nb > 0 && T->pf.last != '\n';
+            X.h2d_ms += T->pf.ms;
+            X.text_bytes[k] = nb;
+            if (k == 0 && (r = prefetch_start(ctx, T, ins[1], false, 1)) != PP_OK) return r;
+            FileDev& fd = X.fd[k];
+            memset(&fd, 0, sizeof fd);
+            fd.text = text;
+            if (nb) r = ftok_lines(ctx, T, k, text, nb, unterminated, B.lines[k], B.tmp[k], X.d_st, &fd, &launches);
+            if (r != PP_OK) {
+                if (T->pf.active) { if (T->pf.th.joinable()) T->pf.th.join(); T->pf.active = false; }
+                return r;
+            }
+        }
+        for (int k = 0; k < 2; ++k)
+            if (X.fd[k].n_lines) CK(cudaMemcpyAsync(T->h_tot + k, X.fd[k].s_al + X.fd[k].n_lines, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&h_st, X.d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        CK(cudaGetLastError());
+        for (int k = 0; k < 2; ++k) X.n_al[k] = X.fd[k].n_lines ? T->h_tot[k] : 0;
+        if (h_st.first_bad[0] != ~0ull || h_st.first_bad[1] != ~0ull) return PP_TOK_HOST;
+        if (X.n_al[0] >= 0x7FFFFFFFull || X.n_al[1] >= 0x7FFFFFFFull) return PP_TOK_HOST;
+        uint64_t cap = 1024;
+        while (cap < 3 * (X.n_al[0] + X.n_al[1]) + 1024) cap <<= 1;
+        if (cap > (1ull << 31)) return PP_TOK_HOST;
+        TRY_ALLOC(B.table.ensure(cap * 16));
+        X.tb.key = B.table.as<unsigned long long>(); X.tb.rep = X.tb.key + cap; X.tb.mask = (uint32_t)(cap - 1);
+        X.slot_val = (uint32_t*)X.tb.key;                                   // (the keys are done with once the slots are verified)
+        CK(cudaMemsetAsync(X.tb.key, 0, cap * 8, s));
+        CK(cudaMemsetAsync(X.tb.rep, 0xFF, cap * 8, s));
+        for (int k = 0; k < 2; ++k)
+            if (X.fd[k].n_lines) k_ftok_intern<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, X.tb, X.d_st);
+        for (int k = 0; k < 2; ++k)
+            if (X.fd[k].n_lines) k_ftok_verify<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[0], X.fd[1], k, X.tb, X.d_st);
+        // the distinct RNAMEs of this GPU, with their bytes
+        uint64_t rcap = std::max<uint64_t>(1024, B.fx_refs.cap / 2 / sizeof(FxRef));
+        for (;;) {
+            TRY_ALLOC(B.fx_refs.ensure(2 * rcap * sizeof(FxRef) + 64));
+            FxRef* d_refs = B.fx_refs.as<FxRef>();
+            unsigned long long* d_n = (unsigned long long*)(d_refs + 2 * rcap - 1);
+            CK(cudaMemsetAsync(d_n, 0, 8, s));
+            for (int k = 0; k < 2; ++k)
+                if (X.fd[k].n_lines) k_fx_refs<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, X.tb, d_refs, d_n, rcap);
+            CK(cudaMemcpyAsync(T->h_tot, d_n, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&h_st, X.d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            CK(cudaGetLastError());
+            if (h_st.collision) return PP_TOK_HOST;
+            const uint64_t nr = T->h_tot[0];
+            if (nr > rcap) { rcap = nr; continue; }
+            X.refs.resize(nr);
+            X.ref_off.assign(nr + 1, 0);
+            if (nr) CK(cudaMemcpyAsync(X.refs.data(), d_refs, nr * sizeof(FxRef), cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            for (uint64_t j = 0; j < nr; ++j) X.ref_off[j + 1] = X.ref_off[j] + X.refs[j].len;
+            X.ref_bytes.resize(X.ref_off[nr] + 1);
+            if (nr) {
+                unsigned long long* d_off = (unsigned long long*)(d_refs + nr);       // (second half of the buffer)
+                uint8_t* d_bytes;
+                TRY_ALLOC(B.fx_stage.ensure(X.ref_off[nr] + 64));
+                d_bytes = B.fx_stage.as<uint8_t>();
+                CK(cudaMemcpyAsync(d_off, X.ref_off.data(), nr * 8, cudaMemcpyHostToDevice, s));
+                k_fx_ref_bytes<<<fx_blocks(nr, 256), 256, 0, s>>>(d_refs, nr, d_off, X.fd[0].text, X.fd[1].text, d_bytes);
+                CK(cudaMemcpyAsync(X.ref_bytes.data(), d_bytes, X.ref_off[nr], cudaMemcpyDeviceToHost, s));
+                CK(cudaStreamSynchronize(s));
+                CK(cudaGetLastError());
+            }
+            break;
+        }
+        X.launches = launches + 6;
+        return PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+    uint64_t n_al_total[2] = {0, 0};
+    for (FxSide& X : S) for (int k = 0; k < 2; ++k) { n_al_total[k] += X.n_al[k]; fs->text_bytes[k] += X.text_bytes[k]; }
+    for (int k = 0; k < 2; ++k) fs->alignments[k] = n_al_total[k];
+    if (n_al_total[0] == 0 || n_al_total[1] == 0) return PP_TOK_HOST;    // "no alignments found in ..." is worded by the host path
+    if (n_al_total[0] >= 0x7FFFFFFFull || n_al_total[1] >= 0x7FFFFFFFull) return PP_TOK_HOST;
+    fs->phase_ms[0] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+
+    // ---- global RNAME ids: numbered by string, in the order the GPUs list them
+    {
+        std::unordered_map<std::string, uint32_t> global;
+        for (FxSide& X : S) {
+            X.ref_global.resize(X.refs.size());
+            for (size_t j = 0; j < X.refs.size(); ++j) {
+                const std::string name((const char*)X.ref_bytes.data() + X.ref_off[j], X.refs[j].len);
+                X.ref_global[j] = make_uint2(X.refs[j].slot, global.emplace(name, (uint32_t)global.size()).first->second);
+            }
+        }
+    }
+    // ---- count what goes where
+    rc = fx_all(S, [&](FxSide& X, int) -> int {
+        pp_ctx* ctx = X.ctx;
+        cudaStream_t s = ctx->stream;
+        TokFilterBufs& B = *X.B;
+        const uint64_t nr = X.ref_global.size();
+        TRY_ALLOC(B.fx_stage.ensure(nr * sizeof(uint2) + 2 * n * (sizeof(FxCount) + sizeof(FxPlan)) + 256));
+        uint2* d_pairs = B.fx_stage.as<uint2>();
+        if (nr) {
+            CK(cudaMemcpyAsync(d_pairs, X.ref_global.data(), nr * sizeof(uint2), cudaMemcpyHostToDevice, s));
+            k_fx_scatter<<<fx_blocks(nr, 256), 256, 0, s>>>(d_pairs, nr, X.slot_val);
+        }
+        FxCount* d_cnt = (FxCount*)(B.fx_stage.as<uint8_t>() + ((nr * sizeof(uint2) + 255) & ~size_t(255)));
+        CK(cudaMemsetAsync(d_cnt, 0, n * sizeof(FxCount), s));
+        for (int k = 0; k < 2; ++k)
+            if (X.fd[k].n_lines) k_fx_count<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, X.tb, n, d_cnt);
+        X.cnt.resize(n);
+        CK(cudaMemcpyAsync(X.cnt.data(), d_cnt, n * sizeof(FxCount), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        CK(cudaGetLastError());
+        X.launches += 3;
+        return PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+    // where every piece goes: at destination d, the pieces of the sources in order; at source g, the destinations in order (file by file)
+    for (uint32_t d = 0; d < n; ++d) {
+        uint64_t at_names = 0, at_bytes = 0, at_recs[2] = {0, 0};
+        for (uint32_t g = 0; g < n; ++g) {
+            const FxCount& c = S[g].cnt[d];
+            at_names += c.names; at_bytes += c.bytes; at_recs[0] += c.recs[0]; at_recs[1] += c.recs[1];
+        }
+        if (at_names >= 0x7FFFFFFFull || at_bytes >= 0xFFFFFFFFull) return PP_TOK_HOST;
+        S[d].rx_names = at_names; S[d].rx_bytes = at_bytes; S[d].rx_recs[0] = at_recs[0]; S[d].rx_recs[1] = at_recs[1];
+    }
+    for (uint32_t g = 0; g < n; ++g) {
+        FxSide& X = S[g];
+        X.plan.assign(n, FxPlan{});
+        X.st_names = X.st_bytes = X.st_recs[0] = X.st_recs[1] = 0;
+        for (uint32_t d = 0; d < n; ++d) {
+            FxPlan& p = X.plan[d];
+            p.stage_name = X.st_names; p.stage_byte = X.st_bytes;
+            X.st_names += X.cnt[d].names; X.st_bytes += X.cnt[d].bytes;
+            for (uint32_t h = 0; h < g; ++h) { p.name_base += S[h].cnt[d].names; p.byte_base += S[h].cnt[d].bytes; }
+        }
+        for (int k = 0; k < 2; ++k)
+            for (uint32_t d = 0; d < n; ++d) { X.plan[d].stage_rec[k] = X.st_recs[0] + X.st_recs[1]; X.st_recs[k] += X.cnt[d].recs[k]; }
+    }
+    auto rec_base = [&](uint32_t g, uint32_t d, int k) { uint64_t b = 0; for (uint32_t h = 0; h < g; ++h) b += S[h].cnt[d].recs[k]; return b; };
+
+    // ---- staging (source) and receive buffers (owner); then the pieces travel
+    rc = fx_all(S, [&](FxSide& X, int) -> int {
+        pp_ctx* ctx = X.ctx;
+        cudaStream_t s = ctx->stream;
+        TokFilterBufs& B = *X.B;
+        auto up = [](uint64_t v) { return (v + 255) & ~uint64_t(255); };
+        const uint64_t st_recs = X.st_recs[0] + X.st_recs[1];
+        const uint64_t o_plan = 0, o_at = up(n * sizeof(FxPlan)), o_names = o_at + up(n * sizeof(FxCount)), o_recs = o_names + up(X.st_names * sizeof(FxName)),
+                       o_bytes = o_recs + up(st_recs * sizeof(FxRec));
+        TRY_ALLOC(B.fx_stage.ensure(o_bytes + X.st_bytes + 64));
+        uint8_t* b = B.fx_stage.as<uint8_t>();
+        X.d_plan = (FxPlan*)(b + o_plan); X.d_at = (FxCount*)(b + o_at); X.s_names = (FxName*)(b + o_names); X.s_recs = (FxRec*)(b + o_recs);
+        X.s_bytes = b + o_bytes;
+        const uint64_t o_pass1 = up(X.n_al[0] + 1), o_ret = o_pass1 + up(X.n_al[1] + 1);
+        TRY_ALLOC(B.fx_home.ensure(o_ret + st_recs + 64));
+        X.pass[0] = B.fx_home.as<uint8_t>(); X.pass[1] = X.pass[0] + o_pass1; X.ret = X.pass[0] + o_ret;
+        const uint64_t o_rb = up(X.rx_names * sizeof(FxName)), o_r0 = o_rb + up(X.rx_bytes + 1), o_r1 = o_r0 + up(X.rx_recs[0] * sizeof(FxRec));
+        TRY_ALLOC(B.fx_rx.ensure(o_r1 + X.rx_recs[1] * sizeof(FxRec) + 64));
+        uint8_t* r = B.fx_rx.as<uint8_t>();
+        X.r_names = (FxName*)r; X.r_bytes = r + o_rb; X.r_recs[0] = (FxRec*)(r + o_r0); X.r_recs[1] = (FxRec*)(r + o_r1);
+        CK(cudaMemcpyAsync(X.d_plan, X.plan.data(), n * sizeof(FxPlan), cudaMemcpyHostToDevice, s));
+        CK(cudaMemsetAsync(X.d_at, 0, n * sizeof(FxCount), s));
+        for (int k = 0; k < 2; ++k)
+            if (X.fd[k].n_lines)
+                k_fx_names<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, X.tb, n, X.d_plan, X.d_at, X.s_names,
+                                                                                                  X.s_bytes, X.slot_val);
+        for (int k = 0; k < 2; ++k)
+            if (X.fd[k].n_lines)
+                k_fx_recs<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, n, X.d_plan, X.d_at, X.slot_val, X.s_recs);
+        CK(cudaStreamSynchronize(s));
+        CK(cudaGetLastError());
+        X.launches += 4;
+        return PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+    rc = fx_all(S, [&](FxSide& X, int g) -> int {
+        for (uint32_t dd = 0; dd < n; ++dd) {
+            const uint32_t d = ((uint32_t)g + dd) % n;                      // (the sources start on different destinations)
+            FxSide& D = S[d];
+            const FxPlan& p = X.plan[d];
+            const FxCount& c = X.cnt[d];
+            int r = fx_copy(X.ctx, D.ctx, D.r_names + p.name_base, X.s_names + p.stage_name, c.names * sizeof(FxName));
+            if (r == PP_OK) r = fx_copy(X.ctx, D.ctx, D.r_bytes + p.byte_base, X.s_bytes + p.stage_byte, c.bytes);
+            for (int k = 0; k < 2 && r == PP_OK; ++k)
+                r = fx_copy(X.ctx, D.ctx, D.r_recs[k] + rec_base((uint32_t)g, d, k), X.s_recs + p.stage_rec[k], c.recs[k] * sizeof(FxRec));
+            if (r != PP_OK) return r;
+        }
+        pp_ctx* ctx = X.ctx;
+        CK(cudaStreamSynchronize(ctx->stream));
+        return PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+    fs->phase_ms[1] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count() - fs->phase_ms[0];
+
+    // ---- owners: intern and verify the names they received, their two Mate arrays, unique pairs
+    rc = fx_all(S, [&](FxSide& X, int) -> int {
+        pp_ctx* ctx = X.ctx;
+        cudaStream_t s = ctx->stream;
+        TokFilterBufs& B = *X.B;
+        uint64_t cap = 1024;
+        while (cap < 2 * X.rx_names + 1024) cap <<= 1;
+        if (cap > (1ull << 31)) return PP_TOK_HOST;
+        auto up = [](uint64_t v) { return (v + 255) & ~uint64_t(255); };
+        const uint64_t o_id = cap * 16, o_m = o_id + up(X.rx_names * 4 + 4);
+        uint64_t o_mate[2][5], end = o_m;
+        for (int k = 0; k < 2; ++k)
+            for (int a = 0; a < 5; ++a) { o_mate[k][a] = end; end += up(X.rx_recs[k] * (a < 4 ? 4 : 1) + 4); }
+        TRY_ALLOC(B.fx_owner.ensure(end + 64));
+        uint8_t* b = B.fx_owner.as<uint8_t>();
+        InternTable t;
+        t.key = (unsigned long long*)b; t.rep = t.key + cap; t.mask = (uint32_t)(cap - 1);
+        uint32_t* id = (uint32_t*)(b + o_id);
+        CK(cudaMemsetAsync(t.key, 0, cap * 8, s));
+        CK(cudaMemsetAsync(t.rep, 0xFF, cap * 8, s));
+        if (X.rx_names) {
+            k_fx_intern<<<fx_blocks(X.rx_names, 256), 256, 0, s>>>(X.r_names, X.rx_names, t, id, X.d_st);
+            k_fx_verify<<<fx_blocks(X.rx_names, 256), 256, 0, s>>>(X.r_names, X.rx_names, X.r_bytes, t, id, X.d_st);
+        }
+        Mate mates[2];
+        for (int k = 0; k < 2; ++k) {
+            MateOut mo;
+            mo.name_id = (uint32_t*)(b + o_mate[k][0]); mo.contig = (uint32_t*)(b + o_mate[k][1]); mo.ref_start = (uint32_t*)(b + o_mate[k][2]);
+            mo.ref_end = (uint32_t*)(b + o_mate[k][3]); mo.flags = b + o_mate[k][4];
+            if (X.rx_recs[k]) k_fx_mates<<<fx_blocks(X.rx_recs[k], 256), 256, 0, s>>>(X.r_recs[k], X.rx_recs[k], id, mo);
+            mates[k].name_id = mo.name_id; mates[k].contig = mo.contig; mates[k].ref_start = mo.ref_start; mates[k].ref_end = mo.ref_end;
+            mates[k].flags = mo.flags; mates[k].cnt = nullptr; mates[k].head = nullptr; mates[k].next = nullptr; mates[k].pass = nullptr;
+            mates[k].n = (uint32_t)X.rx_recs[k];
+        }
+        X.launches += 4;
+        CK(cudaEventRecord(ctx->ev[0], s));
+        int r = filter_begin(ctx, mates, (uint32_t)cap, &X.f, &X.launches);
+        if (r != PP_OK) return r;
+        FStatus h_st;
+        CK(cudaMemcpyAsync(X.pairs, X.f.pairs, 32, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&h_st, X.d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        CK(cudaGetLastError());
+        return h_st.collision ? PP_TOK_HOST : PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+
+    // ---- orientation from the summed pair counts, thresholds by a radix select over all owners (filter.rs:148-186)
+    unsigned long long pairs[4] = {0, 0, 0, 0};
+    for (FxSide& X : S) for (int i = 0; i < 4; ++i) pairs[i] += X.pairs[i];
+    for (int i = 0; i < 4; ++i) res->pairs[i] = pairs[i];
+    int chosen = 0;
+    unsigned long long n_sizes = 0;
+    rc = filter_orientation(c0, prm, pairs, &chosen, &n_sizes);
+    if (rc != PP_OK) return rc;
+    res->orientation = chosen;
+    bool in_range[2];
+    unsigned long long rank[2];
+    filter_ranks(prm, n_sizes, rank, in_range);
+    uint32_t prefix[2] = {0, 0}, done_mask = 0;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+        rc = fx_all(S, [&](FxSide& X, int) { return filter_hist(X.ctx, X.f, (uint32_t)chosen, shift, done_mask, prefix, X.hist, &X.launches); });
+        if (rc != PP_OK) return rc;
+        uint32_t hist[512] = {};
+        for (FxSide& X : S) for (int i = 0; i < 512; ++i) hist[i] += X.hist[i];
+        for (int r = 0; r < 2; ++r) prefix[r] |= filter_pick_digit(hist + r * 256, rank[r]) << shift;
+        done_mask |= 255u << shift;
+    }
+    res->low = in_range[0] ? prefix[0] : 0;
+    res->high = in_range[1] ? prefix[1] : 0;
+
+    // ---- verdicts on the owners, then home to the sources
+    rc = fx_all(S, [&](FxSide& X, int) -> int {
+        pp_ctx* ctx = X.ctx;
+        cudaStream_t s = ctx->stream;
+        filter_pass(ctx, X.f, res->low, res->high, (uint32_t)chosen, &X.launches);
+        CK(cudaMemcpyAsync(X.np, X.f.n_pass, 16, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        CK(cudaGetLastError());
+        return PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+    rc = fx_all(S, [&](FxSide& D, int d) -> int {
+        for (uint32_t gg = 0; gg < n; ++gg) {
+            const uint32_t g = ((uint32_t)d + gg) % n;
+            FxSide& X = S[g];
+            for (int k = 0; k < 2; ++k) {
+                const int r = fx_copy(D.ctx, X.ctx, X.ret + X.plan[(uint32_t)d].stage_rec[k], D.f.m[k].pass + rec_base(g, (uint32_t)d, k),
+                                      X.cnt[(uint32_t)d].recs[k]);
+                if (r != PP_OK) return r;
+            }
+        }
+        pp_ctx* ctx = D.ctx;
+        CK(cudaStreamSynchronize(ctx->stream));
+        return PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+    rc = fx_all(S, [&](FxSide& X, int) -> int {
+        pp_ctx* ctx = X.ctx;
+        const uint64_t st_recs = X.st_recs[0] + X.st_recs[1];
+        if (st_recs) { k_fx_home<<<fx_blocks(st_recs, 256), 256, 0, ctx->stream>>>(X.s_recs, st_recs, X.ret, X.pass[0], X.pass[1]); X.launches++; }
+        CK(cudaStreamSynchronize(ctx->stream));
+        CK(cudaGetLastError());
+        return PP_OK;
+    });
+    if (rc != PP_OK) return rc;
+    uint64_t np[2] = {0, 0};
+    for (FxSide& X : S) { np[0] += X.np[0]; np[1] += X.np[1]; }
+    res->n_pass = np[0] + np[1];
+    for (int k = 0; k < 2; ++k) { fs->pass[k] = np[k]; fs->fail[k] = n_al_total[k] - np[k]; }
+    fs->phase_ms[2] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count() - fs->phase_ms[0] - fs->phase_ms[1];
+
+    // ---- output text: every GPU assembles its piece; the pieces go to their offsets (a regular file) or in range order (anything else)
+    float d2h_ms = 0;
+    for (int k = 0; k < 2; ++k) {
+        if (!outs[k]) continue;
+        const auto t_out = std::chrono::steady_clock::now();
+        rc = fx_all(S, [&](FxSide& X, int) -> int {
+            pp_ctx* ctx = X.ctx;
+            TokState* T = X.T;
+            TokFilterBufs& B = *X.B;
+            cudaStream_t s = ctx->stream;
+            const FileDev& fd = X.fd[k];
+            X.out_n = 0;
+            if (!fd.n_lines) return PP_OK;
+            const uint64_t nl = fd.n_lines;
+            CK(B.table.ensure((nl + 2) * 8));                                // the local intern table is done with: reuse it
+            unsigned long long* out_off = B.table.as<unsigned long long>();
+            k_ftok_outlen<<<fx_blocks(nl + 1, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(fd, X.pass[k], out_off);
+            size_t cub_bytes = 0;
+            CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, out_off, out_off, (int64_t)(nl + 1)));
+            CK(T->cub.ensure(cub_bytes + 256));
+            size_t tbb = T->cub.cap;
+            CK(cub::DeviceScan::ExclusiveSum(T->cub.p, tbb, out_off, out_off, (int64_t)(nl + 1), s));
+            CK(cudaMemcpyAsync(T->h_tot, out_off + nl, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            X.out_n = T->h_tot[0];
+            CK(B.out.ensure(X.out_n + 64));
+            k_ftok_copy<<<fx_blocks(nl * 32, 256), 256, 0, s>>>(fd, X.pass[k], out_off, B.out.as<uint8_t>());
+            CK(cudaStreamSynchronize(s));
+            CK(cudaGetLastError());
+            X.launches += 3;
+            return PP_OK;
+        });
+        if (rc != PP_OK) return rc;
+        std::vector<uint64_t> base(n + 1, 0);
+        for (uint32_t g = 0; g < n; ++g) base[g + 1] = base[g] + S[g].out_n;
+        const uint64_t out_n = base[n];
+        struct stat osb;
+        const bool special = stat(outs[k], &osb) == 0 && !S_ISREG(osb.st_mode);
+        const int ofd = special ? open(outs[k], O_WRONLY) : open(outs[k], O_RDWR | O_CREAT | O_TRUNC, 0666);
+        if (ofd < 0) return c0->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + outs[k] + "\"");
+        std::vector<int> wrc(n, PP_OK), cuda_err(n, 0);
+        bool stream_out = special;
+        if (out_n && !stream_out && ftruncate(ofd, (off_t)out_n) != 0) stream_out = true;
+        if (out_n && stream_out) {
+            for (uint32_t g = 0; g < n && wrc[0] == PP_OK; ++g)
+                if (S[g].out_n) wrc[0] = download_stream(S[g].ctx->device, S[g].T, S[g].B->out.as<uint8_t>(), ofd, S[g].out_n, &cuda_err[0]);
+        } else if (out_n) {
+            // (the one-GPU rule: a mapping only where the file system has room to spare, else pwrite() reports a full disk)
+            struct statvfs vfs;
+            const bool roomy = fstatvfs(ofd, &vfs) == 0 && (uint64_t)vfs.f_bavail * (uint64_t)vfs.f_frsize > 2 * out_n + (64ull << 20);
+            void* map = roomy ? mmap(nullptr, (size_t)out_n, PROT_READ | PROT_WRITE, MAP_SHARED, ofd, 0) : MAP_FAILED;
+            if (map == MAP_FAILED) map = nullptr;
+            std::vector<std::thread> th;
+            for (uint32_t g = 0; g < n; ++g)
+                if (S[g].out_n)
+                    th.emplace_back([&, g] { wrc[g] = download_file(S[g].ctx->device, S[g].T, S[g].B->out.as<uint8_t>(), ofd, (uint8_t*)map, S[g].out_n,
+                                                                    &cuda_err[g], base[g]); });
+            for (auto& t : th) t.join();
+            if (map && munmap(map, (size_t)out_n) != 0 && wrc[0] == PP_OK) wrc[0] = PP_ERR_IO;
+        }
+        int w = PP_OK, ce = 0;
+        for (uint32_t g = 0; g < n; ++g) if (wrc[g] != PP_OK && w == PP_OK) { w = wrc[g]; ce = cuda_err[g]; }
+        if (close(ofd) != 0 && w == PP_OK) w = PP_ERR_IO;
+        d2h_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_out).count();
+        if (w == PP_ERR_IO) return c0->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + outs[k] + "\"");
+        if (w == PP_ERR_CUDA) return c0->fail_cuda((cudaError_t)ce, "filtered SAM download", __FILE__, __LINE__);
+        fs->out_bytes[k] = out_n;
+    }
+    fs->d2h_ms = d2h_ms;
+    for (FxSide& X : S) { fs->launches += X.launches; fs->h2d_ms = std::max(fs->h2d_ms, X.h2d_ms); }
+
+    // ---- filter-polish: every GPU tokenises its ranges for polish, the verdicts become ZP flags; pp_tok_exchange_finish comes next
+    if (fuse) {
+        fuse->rc = PP_TOK_HOST;
+        for (int bits = 4;; bits = 8) {
+            rc = fx_all(S, [&](FxSide& X, int g) -> int {
+                pp_ctx* ctx = X.ctx;
+                TokState* T = X.T;
+                int r = pp_tok_begin(ctx, fuse->fasta, fuse->careful, bits);
+                const uint64_t off[2] = {cuts[0][g], cuts[1][g]}, len[2] = {cuts[0][g + 1] - cuts[0][g], cuts[1][g + 1] - cuts[1][g]};
+                if (r == PP_OK) r = pp_tok_set_ranges(ctx, off, len, 2);
+                if (r != PP_OK) return r;
+                T->expect_total = len[0] + len[1];
+                memset(X.tst, 0, sizeof X.tst);
+                for (int k = 0; k < 2; ++k) {
+                    T->marks.push_back({T->aln_base, T->ops_base, T->blk_base, T->read_base});
+                    const uint64_t a0 = T->aln_base;
+                    r = tok_process(ctx, T, X.fd[k].text, X.fd[k].n, X.fd[k].unterminated != 0, &X.tst[k], true);
+                    if (r == PP_OK && X.tst[k].alignments != X.n_al[k]) r = PP_TOK_HOST;       // (cannot happen: same lines, same rule)
+                    if (r != PP_OK) { T->active = false; return r; }
+                    if (X.n_al[k]) {
+                        k_apply_pass<<<fx_blocks(X.n_al[k], 256), 256, 0, ctx->stream>>>(ctx->b[B_FLAGS].as<uint8_t>() + a0, X.pass[k], X.n_al[k]);
+                        CK(cudaStreamSynchronize(ctx->stream));
+                        CK(cudaGetLastError());
+                    }
+                }
+                T->marks.push_back({T->aln_base, T->ops_base, T->blk_base, T->read_base});
+                return PP_OK;
+            });
+            if (rc == PP_TOK_NEED8 && bits == 4) continue;
+            break;
+        }
+        if (rc == PP_TOK_NEED8) rc = PP_TOK_HOST;
+        if (rc < 0) return rc;
+        if (rc == PP_OK) {
+            memset(fuse->stats, 0, sizeof fuse->stats);
+            for (FxSide& X : S)
+                for (int k = 0; k < 2; ++k) {
+                    fuse->stats[k].alignments += X.tst[k].alignments; fuse->stats[k].reads += X.tst[k].reads; fuse->stats[k].lines += X.tst[k].lines;
+                }
+            fuse->n_aln = n_al_total[0] + n_al_total[1];
+        }
+        fuse->rc = rc;
     }
     fs->total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
     return PP_OK;
