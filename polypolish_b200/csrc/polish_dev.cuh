@@ -71,7 +71,8 @@ struct DevStatus {
     unsigned int n_changes;          // changed positions k_tile appended to the change list (counted beyond its capacity too)
     unsigned int pad1;
 #ifdef PP_TILE_PROF
-    unsigned long long prof[12];     // cycles of thread 0 per phase (A, B, queue, C, D+E), queued reads, tiles, largest queue, depth-walk cycles, walks, tiles with a walk
+    unsigned long long prof[12];     // cycles of thread 0 per phase (A, B, queue, C, D+E), queued reads, tiles, largest queue, depth-walk cycles, walks, tiles with a walk,
+                                     // cycles lane 0 of every warp waited for its chunks' data in phase B
 #endif
 };
 
@@ -791,6 +792,44 @@ struct WalkStage {                                     // per warp: staging of t
     uint32_t key[2][32];                               // alignment indices of the entries being merged, compacted, per run
 };
 
+// Per warp: one chunk of the chunk loop (32 consecutive slots) in shared memory, copied in by one bulk copy per array that
+// completes on the stage's mbarrier.  Bases first: word 24 of lane 31's read, which the trim may load and then not use, is rec[0].
+#define TL_STAGES 2
+struct ChunkStage {
+    uint4 seq[32 * TL_SEQ_QUADS];                      // 4-bit mode: the slots' bases (sseq)
+    TileRec rec[32];                                   // the slots' records (srec)
+};
+
+#if defined(PP_EMULATE)
+// The issuing lane copies; the wait is a warp barrier (the lane that copied has arrived at it).
+static inline void stage_bar_init(unsigned long long*) {}
+static inline void stage_fence() {}
+static inline void stage_expect(unsigned long long*, uint32_t) {}
+static inline void stage_copy(void* dst, const void* src, uint32_t bytes, unsigned long long*) { memcpy(dst, src, bytes); }
+static inline void stage_wait(unsigned long long*, uint32_t) { __syncwarp(); }
+#else
+__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void stage_bar_init(unsigned long long* bar) {   // one arrival per phase: the issuing lane's expect_tx
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n\tfence.mbarrier_init.release.cluster;" ::"r"(smem_addr(bar)) : "memory");
+}
+// Orders this thread's generic shared-memory writes before later bulk copies (async proxy) into the same bytes.
+__device__ __forceinline__ void stage_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void stage_expect(unsigned long long* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void stage_copy(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) {   // 16 B aligned, bytes % 16 == 0
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)) : "memory");
+}
+__device__ __forceinline__ void stage_wait(unsigned long long* bar, uint32_t parity) {
+    uint32_t done;
+    do {
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                     : "=r"(done) : "r"(smem_addr(bar)), "r"(parity) : "memory");
+    } while (!done);
+}
+#endif
+
 struct TileShared {
     int cdiff[TL_T + 4];                               // cover: +1 / -1 at interval ends, after the prefix sum = cover[p]
     uint32_t ex[4][TL_T];                              // A, C, G, T entries that differ from the draft base
@@ -802,8 +841,12 @@ struct TileShared {
         double depth[TL_T];                            // ordered f64 depth, written over the deficit in sub-tiles that walk
     };
     unsigned long long dn[TL_DN_WORDS + 2];            // 4-bit draft codes, 16 per word, position -32 first
-    WalkStage wstage[TL_THREADS / 32];                 // ordered-depth merge staging, one per warp
-    uint32_t queue[TL_QCAP];                           // sorted slots waiting for the two-segment / general walk
+    union {                                            // (phase D only, behind barriers | phase B and the queue)
+        WalkStage wstage[TL_THREADS / 32];             // ordered-depth merge staging, one per warp
+        ChunkStage ring[TL_THREADS / 32][TL_STAGES];   // chunk-loop stages, two per warp; the queue walks use stage 0
+    };
+    unsigned long long ring_bar[TL_THREADS / 32][TL_STAGES];   // one mbarrier per stage
+    uint2 queue[TL_QCAP];                              // (sorted slot, k) of the reads waiting for the two-segment / general walk
     uint32_t qn;
     unsigned long long s_warp[TL_THREADS / 32];
     unsigned long long s_total;
@@ -813,6 +856,7 @@ struct TileShared {
     double inv_k[TL_INV_K + 1];                        // 1.0 / k for small k (the ordered-depth walk divides once per slot otherwise)
     unsigned long long def_k[TL_INV_K + 1];            // depth_deficit(k) for small k (add_interval divides otherwise)
 };
+static_assert(sizeof(TileShared) <= 232448, "k_tile's shared memory: at most 227 KB per CTA on sm_90");
 
 template <int BITS> struct TileCtx {
     const DevData& d;
@@ -983,30 +1027,21 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k)
 
 // The fast path: a 4-bit read of at most 192 bases whose CIGAR is one M / = run.  Its bases were copied into slot order when the
 // dataset was binned - forward strand, base i = nibble i (k_permute_seq) - so slot i's read is the 96 bytes at sseq + 6 i, next to
-// its neighbours' in the tile's list: the six 16-byte loads of a warp's 32 reads cover 3 KB of consecutive memory.  The draft
-// comes from the tile's shared-memory copy through one native funnel shift per 8 bases.
+// its neighbours' in the tile's list: a warp's 32 reads are 3 KB of consecutive memory, which the chunk loop copies into shared
+// memory with one bulk copy.  `w` = the read's 24 words (shared memory; word 24 may be read and is then not used).  The draft comes
+// from the tile's shared-memory copy through one native funnel shift per 8 bases.
 //   pass 1: XOR against the draft four words at a time and only record WHICH words differ - straight-line code, no divergence;
 //   pass 2: the two edge words (partly outside the kept entries or the tile) and the few words that differ (about one word in
-//           two reads) are picked out of the registers again and every differing base is counted.
+//           two reads) are loaded again and every differing base is counted.
 // Returns kept entries, or NONE32 = "take the general walk" (a homopolymer tail of 8+ bases, a read shorter than 8).
-__device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, uint32_t slot, uint32_t k) {
+__device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, const uint32_t* w, uint32_t k) {
     const uint32_t len = r.len_nc & 0xFFFFu;
     const unsigned long long aln = r.aln;
-    const uint4* sp = S.d.sseq + (size_t)slot * TL_SEQ_QUADS;
-    const uint32_t* sp32 = reinterpret_cast<const uint32_t*>(sp);
     if (len < 8) return NONE32;
-    // all six loads of the read are issued before the first one is needed
-    uint4 q[TL_SEQ_QUADS];
-    const uint32_t nq = (len + 31) >> 5;
-#pragma unroll
-    for (int g = 0; g < TL_SEQ_QUADS; ++g) {
-        q[g] = make_uint4(0, 0, 0, 0);
-        if ((uint32_t)g < nq) q[g] = __ldg(sp + g);
-    }
     // ---- trim (alignment.rs:364-378): how many of the last bases equal the last one.  The last 8 bases as one word.
     uint32_t run;
     const uint32_t tw = (len - 8) >> 3;                          // the two words the trim looks at: tw, tw + 1
-    const uint32_t tw0 = __ldg(sp32 + tw), tw1 = __ldg(sp32 + tw + 1);   // (word 24 of the last slot: the pool is padded)
+    const uint32_t tw0 = w[tw], tw1 = w[tw + 1];
     {
         const uint32_t o = len - 8;
         const uint32_t t8 = __funnelshift_r(tw0, tw1, (o & 7) * 4);
@@ -1045,12 +1080,13 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, u
 #pragma unroll
         for (int g = 0; g < TL_SEQ_QUADS; ++g) {
             if ((inner >> (4 * g)) & 15u) {
+                const uint4 q = reinterpret_cast<const uint4*>(w)[g];
                 const uint32_t* dp = dn32 + (i0 + 4 * g);
                 const uint32_t d0 = dp[0], d1 = dp[1], d2 = dp[2], d3 = dp[3], d4 = dp[4];
-                if (q[g].x != __funnelshift_r(d0, d1, sh4)) bits |= 1u << (4 * g);
-                if (q[g].y != __funnelshift_r(d1, d2, sh4)) bits |= 2u << (4 * g);
-                if (q[g].z != __funnelshift_r(d2, d3, sh4)) bits |= 4u << (4 * g);
-                if (q[g].w != __funnelshift_r(d3, d4, sh4)) bits |= 8u << (4 * g);
+                if (q.x != __funnelshift_r(d0, d1, sh4)) bits |= 1u << (4 * g);
+                if (q.y != __funnelshift_r(d1, d2, sh4)) bits |= 2u << (4 * g);
+                if (q.z != __funnelshift_r(d2, d3, sh4)) bits |= 4u << (4 * g);
+                if (q.w != __funnelshift_r(d3, d4, sh4)) bits |= 8u << (4 * g);
             }
         }
         // every base of word m (value wv) that differs from the draft inside [first, lastn]
@@ -1077,12 +1113,7 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, u
         while (mm) {                                           // words that differ (about one word in two reads), clipped edge words
             const uint32_t m = (uint32_t)__ffs((int)mm) - 1;
             mm &= mm - 1;
-            // word m of the read, out of the registers (a select tree: no second trip to memory)
-            const uint32_t g = m >> 2, t4 = m & 3;
-            uint4 qq = q[0];
-#pragma unroll
-            for (int j = 1; j < TL_SEQ_QUADS; ++j) if (g == (uint32_t)j) qq = q[j];
-            count_word(m, t4 == 0 ? qq.x : t4 == 1 ? qq.y : t4 == 2 ? qq.z : qq.w);
+            count_word(m, w[m]);
         }
     };
     if (!one) segment((int)g0, 0, (int)nkept);
@@ -1106,10 +1137,10 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, u
 // one-indel reads, else the general walk.  (Inlined on purpose: as an out-of-line function - half the code size - the calls cost
 // the hot loop its registers and k_tile was measured markedly slower.)
 template <int BITS>
-__device__ __forceinline__ uint32_t slow_walk(const DevData* d, TileShared* sh, uint32_t P0, TileRec r, uint32_t slot, uint32_t k) {
+__device__ __forceinline__ uint32_t slow_walk(const DevData* d, TileShared* sh, uint32_t P0, TileRec r, const uint32_t* seq, uint32_t k) {
     TileCtx<BITS> S{*d, *sh, P0};
     uint32_t nk = NONE32;
-    if (BITS == 4 && (r.flags & TR_FAST1)) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), r, slot, k);
+    if (BITS == 4 && (r.flags & TR_FAST1)) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), r, seq, k);
     if (nk == NONE32) nk = general_walk<BITS>(S, r, k);
     return nk;
 }
@@ -1325,7 +1356,14 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         sh.inv_k[tid] = tid ? __ddiv_rn(1.0, (double)tid) : 0.0;
         sh.def_k[tid] = tid > 1 ? depth_deficit(tid) : 0ull;
     }
+    ChunkStage* const ring = sh.ring[warp];
+    unsigned long long* const bar = sh.ring_bar[warp];
+    if (lane == 0) { stage_bar_init(&bar[0]); stage_bar_init(&bar[1]); }
+    uint32_t parity = 0;                                                       // bit s: the phase stage s completes next (kept across tiles)
     for (;;) {
+        // phase D's and the queue's generic writes to the bytes the ring shares with `wstage` come before the next tile's bulk copies:
+        // every thread fences its own writes, then the barrier
+        stage_fence();
         __syncthreads();                                                       // everyone is done with the previous tile
         if (tid == 0) { sh.tile = atomicAdd(&d.st->ticket, 1u); sh.any_multi = 0; sh.qn = 0; }
         __syncthreads();
@@ -1338,7 +1376,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         pt[0] = clock64();
 #endif
         // The slots of the tile's bins and of the `lb` bins before it - one contiguous range of the binned dataset - and the first two
-        // chunks' records: a chain of four dependent trips to memory (bin bounds, record, its k word, ...) that now runs under phase A.
+        // chunks' copies and SAM indices: a chain of dependent trips to memory (bin bounds, records, k words) that now runs under phase A.
         // (taking the next tile's ticket a tile early, to hide these trips, was measured: the greedy heaviest-first schedule then
         // looks one tile ahead and the kernel's tail grows)
         const uint32_t b0 = P0 >> PP_BIN_SHIFT;
@@ -1346,6 +1384,17 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         const uint32_t hi = d.bin_start[min(b0 + (uint32_t)(TL_T / PP_BIN), d.n_bins)];
         const uint32_t stride = 32u * (TL_THREADS / 32);
         uint32_t c_a = lo + 32u * warp;
+        // lane 0: the records (and, 4-bit, the bases) of the chunk at slot c < hi into stage s; the last chunk of the range is shorter
+        auto issue = [&](uint32_t c, uint32_t s) {
+            const uint32_t n = min(32u, hi - c);
+            stage_expect(&bar[s], n * (uint32_t)(sizeof(TileRec) + (BITS == 4 ? 16 * TL_SEQ_QUADS : 0)));
+            stage_copy(ring[s].rec, d.srec + c, n * (uint32_t)sizeof(TileRec), &bar[s]);
+            if (BITS == 4) stage_copy(ring[s].seq, d.sseq + (size_t)c * TL_SEQ_QUADS, n * 16u * TL_SEQ_QUADS, &bar[s]);
+        };
+        if (lane == 0) {
+            if (c_a < hi) issue(c_a, 0);
+            if (c_a + stride < hi) issue(c_a + stride, 1);
+        }
         // Only two words per lane travel from one round of the chunk loop to the next - the SAM index of the NEXT chunk's record (what
         // its k word is gathered with) and that k word.  (Carrying whole records two chunks ahead cost 16 registers the fast walk does
         // not have: they lived on the stack, and every round began with their reloads from local memory.)
@@ -1353,7 +1402,6 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         uint32_t k_a = 0;
         const uint32_t aln_a = __ldg(&d.srec[min(c_a + lane, last_slot)].aln);
         uint32_t aln_b = __ldg(&d.srec[min(c_a + stride + lane, last_slot)].aln);
-        if (BITS == 4 && c_a + lane < hi) PP_PREFETCH_L2(reinterpret_cast<const uint8_t*>(d.sseq + (size_t)(c_a + lane) * TL_SEQ_QUADS));
         // ---- phase A: clear the counters, stage the draft as 4-bit codes
         {
             uint4* z = reinterpret_cast<uint4*>(sh.cdiff);
@@ -1380,37 +1428,47 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 }
             }
         }
-        if (c_a + lane < hi) k_a = d.kf[aln_a];                // (the record has arrived while the counters were cleared)
+        if (c_a + lane < hi) k_a = d.kf[aln_a];                // (the SAM index has arrived while the counters were cleared)
         __syncthreads();
 #ifdef PP_TILE_PROF
         pt[1] = clock64();
 #endif
         // ---- phase B: every alignment that can touch the tile: the slots of the tile's bins and of the `lb` bins before it - one
-        // contiguous range of the binned dataset.  Warps take chunks of 32 consecutive slots round robin: records and bases stream
-        // in coalesced; the only gather is the 4-byte "k / contributes" word of the current options, fetched one chunk ahead.
+        // contiguous range of the binned dataset.  Warps take chunks of 32 consecutive slots round robin.  A chunk's records and bases
+        // are 1 KB + 3 KB of consecutive memory: lane 0 copies them into one of the warp's two stages in shared memory one chunk ahead,
+        // so the walk starts on data that is already there.  The only gather is the 4-byte "k / contributes" word of the current
+        // options, fetched one chunk ahead.
         {
             // reads that need more than the plain fast walk (one indel: the two-segment fast walk; more indels, long reads,
             // homopolymer tails: the general walk) go to a block-wide queue and are dealt to the warps after the chunk
             // loop, which therefore runs the same straight-line code on every lane
+#ifdef PP_TILE_PROF
+            unsigned long long wait_cyc = 0;
+#endif
+            uint32_t s = 0;                                    // the stage of chunk c_a
             while (c_a < hi) {
                 const uint32_t c_b = c_a + stride, c_c = c_b + stride;
-                // next chunk: its k word (its SAM index arrived during the previous round); the chunk after: its SAM index (which also
-                // brings the 32-byte record into L2); this chunk: its records, requested together with the bases
+                // next chunk: its k word (its SAM index arrived during the previous round); the chunk after: its SAM index
                 uint32_t k_b = 0;
                 if (c_b + lane < hi) k_b = d.kf[aln_b];
                 const uint32_t aln_c = __ldg(&d.srec[min(c_c + lane, last_slot)].aln);
-                const TileRec rec_a = load_srec(d, min(c_a + lane, last_slot));
-                if (BITS == 4 && c_b + lane < hi) {                                    // and its bases towards L2 (contiguous: exact lines)
-                    const uint8_t* nsp = reinterpret_cast<const uint8_t*>(d.sseq + (size_t)(c_b + lane) * TL_SEQ_QUADS);
-                    PP_PREFETCH_L2(nsp);
-                }
+#ifdef PP_TILE_PROF
+                const long long w0 = clock64();
+#endif
+                stage_wait(&bar[s], (parity >> s) & 1u);
+                parity ^= 1u << s;
+#ifdef PP_TILE_PROF
+                if (lane == 0) wait_cyc += (unsigned long long)(clock64() - w0);
+#endif
+                const TileRec rec_a = ring[s].rec[lane];      // (lanes past hi: bytes of an earlier chunk, not used)
+                const uint32_t* const seq_a = reinterpret_cast<const uint32_t*>(ring[s].seq + lane * TL_SEQ_QUADS);
                 const uint32_t i = c_a + lane;
                 bool defer = false;
                 if (i < hi) {
                     if (k_a == 0) d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, 0u, 1u);           // adds nothing under these options
                     else {
                         uint32_t nk = NONE32;
-                        if (BITS == 4 && (rec_a.flags & (TR_FAST | TR_FAST1)) == TR_FAST) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), rec_a, i, k_a);   // (one-indel reads wait for the queue: the chunk loop stays uniform)
+                        if (BITS == 4 && (rec_a.flags & (TR_FAST | TR_FAST1)) == TR_FAST) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), rec_a, seq_a, k_a);   // (one-indel reads wait for the queue: the chunk loop stays uniform)
                         if (nk == NONE32) defer = true;
                         else d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, nk, k_a);
                     }
@@ -1418,14 +1476,19 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 if (defer) {
                     const uint32_t qi = atomicAdd(&sh.qn, 1u);
                     if (qi < TL_QCAP) {
-                        sh.queue[qi] = i;
+                        sh.queue[qi] = make_uint2(i, k_a);
                         PP_PREFETCH_L2(d.cigar_ops + rec_a.cigar_off);                  // what the general walk will chase
                         PP_PREFETCH_L2(d.seq_pool + (size_t)rec_a.seq_off * (BITS == 4 ? 16 : 32));
                     } else                                                             // (a tile with more than TL_QCAP such reads)
-                        d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, slow_walk<BITS>(&d, &sh, P0, rec_a, i, k_a), k_a);
+                        d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, slow_walk<BITS>(&d, &sh, P0, rec_a, seq_a, k_a), k_a);
                 }
-                c_a = c_b; aln_b = aln_c; k_a = k_b;
+                __syncwarp();                                  // every lane is done with stage s: refill it with the chunk after next
+                if (lane == 0 && c_c < hi) issue(c_c, s);
+                c_a = c_b; aln_b = aln_c; k_a = k_b; s ^= 1u;
             }
+#ifdef PP_TILE_PROF
+            if (lane == 0 && wait_cyc) atomicAdd(&d.st->prof[11], wait_cyc);
+#endif
         }
         __syncthreads();
 #ifdef PP_TILE_PROF
@@ -1436,18 +1499,30 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             // the union of their paths (measured: 38 queued reads per tile took a third of the tile's time on two warps).  So the
             // queue is dealt one read per WARP first - lane 0 of every warp, then lane 1, ... - and the walks overlap instead.
             const uint32_t qn = min(sh.qn, (uint32_t)TL_QCAP);
+            // The entry carries k, and the record and the bases (which the two-segment fast walk reads from this lane's place in its
+            // warp's stage 0, free after the chunk loop) are both addressed by the slot: all of them are requested together.  (A read
+            // for the general walk has no bases in `sseq`: its 96 bytes are staged and never read.)
             for (uint32_t qi = lane * (TL_THREADS / 32) + warp; qi < qn; qi += TL_THREADS) {
-                const uint32_t i = sh.queue[qi];
+                const uint2 q = sh.queue[qi];
+                const uint32_t i = q.x, k = q.y;
                 const TileRec r = load_srec(d, i);
-                const uint32_t k = d.kf[r.aln];
-                d.wrec[i] = make_uint4(r.aln, r.gstart, slow_walk<BITS>(&d, &sh, P0, r, i, k), k);
+                uint4* const seq = ring[0].seq + lane * TL_SEQ_QUADS;
+                if (BITS == 4) {
+                    uint4 b[TL_SEQ_QUADS];
+#pragma unroll
+                    for (int g = 0; g < TL_SEQ_QUADS; ++g) b[g] = __ldg(d.sseq + (size_t)i * TL_SEQ_QUADS + g);
+#pragma unroll
+                    for (int g = 0; g < TL_SEQ_QUADS; ++g) seq[g] = b[g];
+                }
+                d.wrec[i] = make_uint4(r.aln, r.gstart, slow_walk<BITS>(&d, &sh, P0, r, reinterpret_cast<const uint32_t*>(seq), k), k);
             }
             // the long list: alignments of more than TL_LONG_E entries, looked at by every tile
             for (uint32_t i = long_lo + tid; i < long_hi; i += TL_THREADS) {
                 const TileRec r = load_srec(d, i);
                 const unsigned long long e_end = (unsigned long long)r.gstart + r.E;
                 const uint32_t k = d.kf[r.aln];
-                if (k != 0 && e_end > P0 && r.gstart < P0 + (uint32_t)TL_T) d.wrec[i] = make_uint4(r.aln, r.gstart, slow_walk<BITS>(&d, &sh, P0, r, i, k), k);
+                // (k_bin marks no long alignment TR_FAST1: the general walk is the only one they take)
+                if (k != 0 && e_end > P0 && r.gstart < P0 + (uint32_t)TL_T) d.wrec[i] = make_uint4(r.aln, r.gstart, general_walk<BITS>(S, r, k), k);
             }
         }
         __syncwarp();          // lanes that had a queued read rejoin their warp here: without it the warp may run phase C in two groups

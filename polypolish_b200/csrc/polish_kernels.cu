@@ -482,9 +482,10 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
         CK(cudaGetLastError());
         const DevStatus hs = *ctx->h_status;
 #ifdef PP_TILE_PROF
-        fprintf(stderr, "[tile prof] tiles %llu; cycles/tile: A %.0f B %.0f queue %.0f C %.0f D+E %.0f; queued reads/tile %.1f (max %llu)\n", hs.prof[6],
+        fprintf(stderr, "[tile prof] tiles %llu; cycles/tile: A %.0f B %.0f queue %.0f C %.0f D+E %.0f; queued reads/tile %.1f (max %llu); "
+                "chunk wait/tile/warp %.0f\n", hs.prof[6],
                 (double)hs.prof[0] / hs.prof[6], (double)hs.prof[1] / hs.prof[6], (double)hs.prof[2] / hs.prof[6], (double)hs.prof[3] / hs.prof[6],
-                (double)hs.prof[4] / hs.prof[6], (double)hs.prof[5] / hs.prof[6], hs.prof[7]);
+                (double)hs.prof[4] / hs.prof[6], (double)hs.prof[5] / hs.prof[6], hs.prof[7], (double)hs.prof[11] / hs.prof[6] / (TL_THREADS / 32));
         fprintf(stderr, "[tile prof] depth walks %llu (%.2f per tile, %llu tiles with one), %.0f cycles each\n", hs.prof[9], (double)hs.prof[9] / hs.prof[6], hs.prof[10],
                 hs.prof[9] ? (double)hs.prof[8] / hs.prof[9] : 0.0);
 #endif
