@@ -801,12 +801,12 @@ struct ChunkStage {
 };
 
 #if defined(PP_EMULATE)
-// The issuing lane copies; the wait is a warp barrier (the lane that copied has arrived at it).
-static inline void stage_bar_init(unsigned long long*) {}
+// The CPU emulator's strict model of the bulk copies and mbarriers (tests/emu/cuda_emu.h): a protocol error fails there.
+static inline void stage_bar_init(unsigned long long* bar) { emu::ring_init(bar); }
 static inline void stage_fence() {}
-static inline void stage_expect(unsigned long long*, uint32_t) {}
-static inline void stage_copy(void* dst, const void* src, uint32_t bytes, unsigned long long*) { memcpy(dst, src, bytes); }
-static inline void stage_wait(unsigned long long*, uint32_t) { __syncwarp(); }
+static inline void stage_expect(unsigned long long* bar, uint32_t bytes) { emu::ring_expect(bar, bytes); }
+static inline void stage_copy(void* dst, const void* src, uint32_t bytes, unsigned long long* bar) { emu::ring_copy(dst, src, bytes, bar); }
+static inline void stage_wait(unsigned long long* bar, uint32_t parity) { emu::ring_wait(bar, parity); }
 #else
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void stage_bar_init(unsigned long long* bar) {   // one arrival per phase: the issuing lane's expect_tx

@@ -1,6 +1,7 @@
 // emu_changes.cpp — the polish kernels of polypolish_b200/csrc/polish_dev.cuh on the CPU (tests/emu/cuda_emu.h) with the change
 // report recorded: k_tile<BITS, true>'s change list, then k_allele_strings over it, then the product's row formatter (debug_rows.h).
-// The same launch sequence as emu_polish.cpp, plus those steps.
+// On request also the whole --debug TSV: k_tile's record of every position (vp.dbg), k_allele_strings over the positions that have
+// other alleles or emit a node, and the same formatter.  The same launch sequence as emu_polish.cpp, plus those steps.
 // TEST INFRASTRUCTURE: built and used by tests/test_emu_changes.py only; nothing in polypolish_b200/ links or loads this.
 #include "cuda_emu.h"
 
@@ -21,7 +22,7 @@ void init_comp_table() {
 
 template <int BITS>
 int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles, bool global_k,
-        uint64_t* err_out, const char* const* names, std::string* changes) {
+        uint64_t* err_out, const char* const* names, std::string* changes, std::string* debug) {
     const uint64_t G = c->off[c->n_contigs], n_aln = a->n_aln;
     const uint32_t n_tiles = (uint32_t)((G + TL_T - 1) / TL_T), n_bins = (uint32_t)((G + PP_BIN - 1) >> PP_BIN_SHIFT);
     const size_t padG = (size_t)n_tiles * TL_T + 16;
@@ -69,7 +70,8 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
     VoteParams vp;
     vp.n_chunks = n_tiles; vp.out = out.data(); vp.out_cap = out_cap; vp.out_off = out_off.data(); vp.changed = changed.data();
     vp.zero_depth = zero.data(); vp.total_depth = tdepth.data(); vp.res = resv.data(); vp.rec_at = rec_at.data(); vp.chunk_delta = chunk_delta.data();
-    vp.dbg = nullptr;
+    std::vector<pp_debug_pos> dbg(debug ? G + 1 : 0);
+    vp.dbg = debug ? dbg.data() : nullptr;
     // the change list, with room for every position: it never overflows here
     std::vector<pp_debug_pos> chg(G + 1);
     std::vector<uint32_t> chg_pos(G + 1);
@@ -133,6 +135,27 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
             const uint32_t ctg = (uint32_t)(std::upper_bound(c->off, c->off + c->n_contigs + 1, (uint64_t)chg_pos[i]) - c->off) - 1;
             rows.add(*changes, names[ctg], chg_pos[i] - c->off[ctg], chg[i], pool.data() + off[i]);
         }
+        if (debug) {                                        // every position: the strings of those with other alleles or a node
+            std::vector<uint32_t> at;
+            for (uint64_t p = 0; p < G; ++p)
+                if (dbg[p].n_other || dbg[p].new_node != 0xFFFFFFFFu) at.push_back((uint32_t)p);
+            const uint32_t na = (uint32_t)at.size();
+            std::vector<uint8_t> dpool(1);
+            std::vector<unsigned long long> doff(na + 1);
+            for (int attempt = 0; attempt < 2; ++attempt) {
+                used = 0;
+                emu::launch(2, 64, 0, [&] { allele_strings_body<BITS>(oc, at.data(), dbg.data(), true, na, dpool.data(), dpool.size(), &used, doff.data()); });
+                if (used <= dpool.size()) break;
+                dpool.resize(used);
+            }
+            *debug = pp::DEBUG_HEADER;
+            size_t k = 0;
+            for (uint32_t ci = 0; ci < c->n_contigs; ++ci)
+                for (uint64_t p = c->off[ci]; p < c->off[ci + 1]; ++p) {
+                    const uint8_t* al = (k < at.size() && at[k] == p) ? dpool.data() + doff[k++] : nullptr;
+                    rows.add(*debug, names[ci], p - c->off[ci], dbg[p], al);
+                }
+        }
     }
     *err_out = st.err;
     res->out_len = st.out_len;
@@ -155,17 +178,26 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
 }  // namespace
 
 // The polish kernels on the CPU with the change report: names = the contigs' names; *changes_tsv (free with emu_free) receives
-// the bytes `polish --changes` writes.  grid_tiles = CTAs of k_tile (they share tiles through the ticket, like on the device).
-extern "C" int emu_polish_changes(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,
-                                  unsigned long long* err_code, const char* const* names, char** changes_tsv) {
+// the bytes `polish --changes` writes, and *debug_tsv, when debug_tsv is not null, the bytes `polish --debug` writes.
+// grid_tiles = CTAs of k_tile (they share tiles through the ticket, like on the device).
+extern "C" int emu_polish_report(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,
+                                 unsigned long long* err_code, const char* const* names, char** changes_tsv, char** debug_tsv) {
     init_comp_table();
     uint64_t err = 0;
-    std::string tsv;
-    int rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, false, &err, names, &tsv) : run<8>(c, a, prm, res, grid_tiles, false, &err, names, &tsv);
-    if (rc == 100) rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, true, &err, names, &tsv) : run<8>(c, a, prm, res, grid_tiles, true, &err, names, &tsv);
+    std::string tsv, dtsv;
+    std::string* dp = debug_tsv ? &dtsv : nullptr;
+    int rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, false, &err, names, &tsv, dp) : run<8>(c, a, prm, res, grid_tiles, false, &err, names, &tsv, dp);
+    if (rc == 100) rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, true, &err, names, &tsv, dp) : run<8>(c, a, prm, res, grid_tiles, true, &err, names, &tsv, dp);
     if (err_code) *err_code = err;
     *changes_tsv = strdup(tsv.c_str());
+    if (debug_tsv) *debug_tsv = strdup(dtsv.c_str());
     return rc;
+}
+
+// The change report only (the entry point tests/emu_changes_lib.py binds).
+extern "C" int emu_polish_changes(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,
+                                  unsigned long long* err_code, const char* const* names, char** changes_tsv) {
+    return emu_polish_report(c, a, prm, res, grid_tiles, err_code, names, changes_tsv, nullptr);
 }
 
 extern "C" void emu_free(void* p) { free(p); }

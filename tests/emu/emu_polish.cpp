@@ -10,6 +10,7 @@
 
 static int g_last_global_k = 0;
 static unsigned g_last_max_ext = 0, g_last_n_long = 0;
+static std::vector<uint32_t> g_last_bin_start, g_last_sval, g_last_tile_order;
 
 namespace {
 
@@ -85,6 +86,8 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
     d.max_ext = st.max_ext;
     g_last_max_ext = st.max_ext;
     g_last_n_long = bin_start[n_bins + 1] - bin_start[n_bins];
+    g_last_bin_start.assign(bin_start.begin(), bin_start.begin() + n_bins + 2);
+    g_last_sval.assign(sval.begin(), sval.begin() + d.n_slots);
     if (d.n_slots) {
         emu::launch((d.n_slots + 255) / 256, 256, 0, [&] { permute_body(d); });
         if (BITS == 4) emu::launch((unsigned)(((uint64_t)d.n_slots * TL_SEQ_QUADS + 255) / 256), 256, 0, [&] { permute_seq_body(d); });
@@ -98,6 +101,7 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
         for (uint32_t i = 0; i < n_tiles; ++i) torder[i] = tindex[o[i]];
     }
     d.tile_order = torder.data();
+    g_last_tile_order.assign(torder.begin(), torder.begin() + n_tiles);
     // ---- per call
     if (n_aln && global_k) emu::launch(2, 256, 0, [&] { k_classify_multi(d); });
     if (n_aln)
@@ -136,6 +140,15 @@ extern "C" int emu_last_global_k() { return g_last_global_k; }
 // back) and the alignments of the long list.
 extern "C" unsigned emu_last_max_ext() { return g_last_max_ext; }
 extern "C" unsigned emu_last_n_long() { return g_last_n_long; }
+// ... and how it laid the alignments out for k_tile: bin_start[0 .. n_bins + 1] (the long list is [bin_start[n_bins],
+// bin_start[n_bins + 1])), the alignment in each slot (sval[0 .. n_slots)) and the order the tiles are dealt in (tile_order).
+// With null arrays: the sizes only.
+extern "C" void emu_last_layout(uint32_t* n_bins, uint32_t* n_slots, uint32_t* n_tiles, uint32_t* bin_start, uint32_t* sval, uint32_t* tile_order) {
+    *n_bins = (uint32_t)g_last_bin_start.size() - 2; *n_slots = (uint32_t)g_last_sval.size(); *n_tiles = (uint32_t)g_last_tile_order.size();
+    if (bin_start) std::copy(g_last_bin_start.begin(), g_last_bin_start.end(), bin_start);
+    if (sval) std::copy(g_last_sval.begin(), g_last_sval.end(), sval);
+    if (tile_order) std::copy(g_last_tile_order.begin(), g_last_tile_order.end(), tile_order);
+}
 
 // The polish kernels on the CPU.  grid_tiles = CTAs of k_tile (they share tiles through the ticket, like on the device).
 extern "C" int emu_polish(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,
