@@ -402,10 +402,11 @@ __device__ __forceinline__ void bin_body(const DevData& d) {
                 const bool fast = BITS == 4 && ncig == 1 && (f0 == PP_OP_M || f0 == PP_OP_EQ) && len <= TL_FAST_LEN;
                 uint32_t flags = ((fl & PP_FLAG_RC) ? TR_RC : 0u) | (fast ? TR_FAST : 0u) | (is_long ? TR_LONG : 0u);
                 if (BITS == 4 && ncig == 3 && len <= TL_FAST_LEN && !is_long) {
-                    // one insertion or one deletion between two match runs: aM bI cM / aM bD cM with a trim that stays in the last run
+                    // one insertion or one deletion between two match runs: aM bI cM / aM bD cM (the fast walk hands the read to the
+                    // general walk when its trim reaches past the last run)
                     const uint32_t o1 = ops[1] & 15u, o2 = ops[2] & 15u, la = ops[0] >> 4, lb2 = ops[1] >> 4, lc = ops[2] >> 4;
                     if ((f0 == PP_OP_M || f0 == PP_OP_EQ) && (o1 == PP_OP_I || o1 == PP_OP_D) && (o2 == PP_OP_M || o2 == PP_OP_EQ) &&
-                        la >= 1 && la <= 255 && lb2 >= 1 && lb2 <= 4095 && lc >= 9)
+                        la >= 1 && la <= 255 && lb2 >= 1 && lb2 <= 4095 && lc >= 1)
                         flags |= TR_FAST | TR_FAST1 | (la << 8) | (lb2 << 16) | (o1 == PP_OP_D ? 1u << 28 : 0u);
                 }
                 uint4* dst = reinterpret_cast<uint4*>(d.recs + aln);
@@ -841,12 +842,12 @@ struct TileShared {
         double depth[TL_T];                            // ordered f64 depth, written over the deficit in sub-tiles that walk
     };
     unsigned long long dn[TL_DN_WORDS + 2];            // 4-bit draft codes, 16 per word, position -32 first
-    union {                                            // (phase D only, behind barriers | phase B and the queue)
+    union {                                            // (phase D only, behind barriers | phase B)
         WalkStage wstage[TL_THREADS / 32];             // ordered-depth merge staging, one per warp
-        ChunkStage ring[TL_THREADS / 32][TL_STAGES];   // chunk-loop stages, two per warp; the queue walks use stage 0
+        ChunkStage ring[TL_THREADS / 32][TL_STAGES];   // chunk-loop stages, two per warp
     };
     unsigned long long ring_bar[TL_THREADS / 32][TL_STAGES];   // one mbarrier per stage
-    uint2 queue[TL_QCAP];                              // (sorted slot, k) of the reads waiting for the two-segment / general walk
+    uint2 queue[TL_QCAP];                              // (sorted slot, k) of the reads waiting for the general walk
     uint32_t qn;
     unsigned long long s_warp[TL_THREADS / 32];
     unsigned long long s_total;
@@ -1025,15 +1026,21 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k)
     return nkept;
 }
 
-// The fast path: a 4-bit read of at most 192 bases whose CIGAR is one M / = run.  Its bases were copied into slot order when the
-// dataset was binned - forward strand, base i = nibble i (k_permute_seq) - so slot i's read is the 96 bytes at sseq + 6 i, next to
-// its neighbours' in the tile's list: a warp's 32 reads are 3 KB of consecutive memory, which the chunk loop copies into shared
-// memory with one bulk copy.  `w` = the read's 24 words (shared memory; word 24 may be read and is then not used).  The draft comes
-// from the tile's shared-memory copy through one native funnel shift per 8 bases.
-//   pass 1: XOR against the draft four words at a time and only record WHICH words differ - straight-line code, no divergence;
-//   pass 2: the two edge words (partly outside the kept entries or the tile) and the few words that differ (about one word in
-//           two reads) are loaded again and every differing base is counted.
-// Returns kept entries, or NONE32 = "take the general walk" (a homopolymer tail of 8+ bases, a read shorter than 8).
+// The fast path: a 4-bit read of at most 192 bases whose CIGAR is one M / = run, or two of them around one insertion or deletion
+// (TR_FAST1: aM bI cM / aM bD cM).  Its bases were copied into slot order when the dataset was binned - forward strand, base i =
+// nibble i (k_permute_seq) - so slot i's read is the 96 bytes at sseq + 6 i, next to its neighbours' in the tile's list: a warp's 32
+// reads are 3 KB of consecutive memory, which the chunk loop copies into shared memory with one bulk copy.  `w` = the read's 24 words
+// (shared memory; word 24 may be read and is then not used).  The draft comes from the tile's shared-memory copy through one native
+// funnel shift per 8 bases.  The read's single-base entries are at most two segments of the read, each at its own draft offset: A =
+// the first match run, B = the last one of a one-indel read (empty for a plain read).
+//   pass 1: XOR against the draft four words at a time and only record WHICH words differ - straight-line code, no divergence.  A
+//           group of four words compares at segment A's offset if it holds a whole word of A, else at B's;
+//   pass 2: the edge words (partly outside a segment or the tile: among them the words at the boundary and those with inserted
+//           bases), the whole words of B in a group compared at A's offset, and the few words that differ (about one word in two
+//           reads) are loaded again and every differing base is counted, once per segment the word holds.
+// Only the insertion's allele, the deletion's "-" entries and pass 2 diverge between plain and one-indel reads.
+// Returns kept entries, or NONE32 = "take the general walk" (a homopolymer tail of 8+ bases or one longer than the last match run, a
+// read shorter than 8).
 __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, const uint32_t* w, uint32_t k) {
     const uint32_t len = r.len_nc & 0xFFFFu;
     const unsigned long long aln = r.aln;
@@ -1050,99 +1057,113 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, c
         if (nz == 0) return NONE32;                            // 8+ equal bases at the end: the general walk counts them
         run = 7u - ((31u - (uint32_t)__clz((int)nz)) >> 2);
     }
-    // one insertion / deletion between two match runs (TR_FAST1): the last run has 9+ entries, so the trim (at most 8) stays in it
     const bool one = r.flags & TR_FAST1;
-    const uint32_t ia = (r.flags >> 8) & 0xFFu, ib = (r.flags >> 16) & 0xFFFu;
+    const uint32_t ia = (r.flags >> 8) & 0xFFu, ib = (r.flags >> 16) & 0xFFFu;            // (0 for a plain read)
     const bool is_del = (r.flags >> 28) & 1u;
-    const uint32_t E = one ? (is_del ? len + ib : len - ib) : len;
-    const uint32_t nkept = E - run - 1;                         // run < 8 < entries of the last run
+    // The general walk's trim stops at the start of the last match run: before it, a D entry carries no inserted base (its `pend` is
+    // 0, so it never counts) and the entry before an I carries the inserted bases (pend != 0).  So the trim is `run` while run <= lc;
+    // beyond that the 8-base window has looked past the run, and the general walk takes the read.  (A plain read: lc = len >= 8 > run.)
+    const uint32_t lc = len - ia - (is_del ? 0u : ib);
+    if (run > lc) return NONE32;
+    const uint32_t E = is_del ? len + ib : len - ib;
+    const uint32_t nkept = E - run - 1;                         // >= a - 1 (I) / a + b - 1 (D): segment A is always kept whole
     if ((unsigned long long)r.gstart + nkept > r.cend) { report_error(S.d.st, aln, ERR_OOB); return 0; }
     S.add_interval(r.gstart, nkept, k);
     const long long g0 = (long long)r.gstart - (long long)S.P0;
     if (g0 >= (long long)TL_T || g0 + (long long)nkept <= 0) return nkept;
     const uint32_t* dn32 = reinterpret_cast<const uint32_t*>(S.sh.dn);
-    // Bases [b_lo, b_hi) of the read are single-base entries at tile-relative positions relq + base: XOR against the draft 8 bases per
-    // native funnel shift and only record WHICH words differ (straight-line code), then revisit those words and the two edge words.
-    auto segment = [&](int relq, int b_lo, int b_hi) {
-        const int lo_b = max(b_lo, -relq), hi_b = min(b_hi, (int)TL_T - relq);
-        if (hi_b <= lo_b) return;
-        const uint32_t first = (uint32_t)lo_b, lastn = (uint32_t)(hi_b - 1);       // first / last valid base
-        const uint32_t m_first = first >> 3, m_last = lastn >> 3;
-        const uint32_t fmask = 0xFFFFFFFFu << ((first & 7) * 4), lmask = 0xFFFFFFFFu >> ((7 - (lastn & 7)) * 4);
-        // an edge word needs its own visit only when it is partly outside [first, lastn] (a read that starts inside the tile starts
-        // on a word boundary: its first word is a whole word like any other)
-        const uint32_t emask = ((first & 7) ? 1u << m_first : 0u) | ((lastn & 7) != 7 ? 1u << m_last : 0u);
-        const uint32_t inner = ((2u << m_last) - (1u << m_first)) & ~emask;        // whole words
-        const int o0 = relq + TL_DN_HALO;                       // nibble offset of word 0 in the staged draft
-        const int i0 = o0 >> 3;                                 // floor; i0 + m >= 0 for every word of a group that holds a valid word
-        const uint32_t sh4 = (uint32_t)(o0 & 7) * 4;
-        uint32_t bits = 0;
+    // Segment s: read bases [lo, hi) are single-base entries at tile-relative positions relq + base, clipped to the tile.
+    //   plain: A = [0, nkept);  aM bI cM: A = [0, a - 1), entry a - 1 carries 1 + b bases (an "other" allele), B = [a + b, nkept + b) at
+    //   relq - b;  aM bD cM: A = [0, a), b "-" entries, B = [a, nkept - b) at relq + b.
+    int relq[2], lo[2], hi[2], i0[2];
+    uint32_t sh4[2], inner[2], edge[2];
+    relq[0] = (int)g0;
+    relq[1] = (int)g0 + (is_del ? (int)ib : -(int)ib);
+    lo[0] = 0;
+    hi[0] = !one ? (int)nkept : (int)ia - (is_del ? 0 : 1);
+    lo[1] = one ? (int)(ia + (is_del ? 0u : ib)) : 0;
+    hi[1] = one ? (int)nkept + (is_del ? -(int)ib : (int)ib) : 0;
 #pragma unroll
-        for (int g = 0; g < TL_SEQ_QUADS; ++g) {
-            if ((inner >> (4 * g)) & 15u) {
-                const uint4 q = reinterpret_cast<const uint4*>(w)[g];
-                const uint32_t* dp = dn32 + (i0 + 4 * g);
-                const uint32_t d0 = dp[0], d1 = dp[1], d2 = dp[2], d3 = dp[3], d4 = dp[4];
-                if (q.x != __funnelshift_r(d0, d1, sh4)) bits |= 1u << (4 * g);
-                if (q.y != __funnelshift_r(d1, d2, sh4)) bits |= 2u << (4 * g);
-                if (q.z != __funnelshift_r(d2, d3, sh4)) bits |= 4u << (4 * g);
-                if (q.w != __funnelshift_r(d3, d4, sh4)) bits |= 8u << (4 * g);
-            }
+    for (int s = 0; s < 2; ++s) {
+        lo[s] = max(lo[s], -relq[s]);
+        hi[s] = min(hi[s], (int)TL_T - relq[s]);
+        const int o0 = relq[s] + TL_DN_HALO;                   // nibble offset of word 0 in the staged draft
+        i0[s] = o0 >> 3;                                        // floor; i0 + m >= 0 for every word of a group that holds a valid word
+        sh4[s] = (uint32_t)(o0 & 7) * 4;
+        inner[s] = edge[s] = 0;
+        if (hi[s] > lo[s]) {
+            const uint32_t first = (uint32_t)lo[s], lastn = (uint32_t)(hi[s] - 1), m_first = first >> 3, m_last = lastn >> 3;
+            // an edge word needs its own visit only when it is partly outside [first, lastn] (a read that starts inside the tile starts
+            // on a word boundary: its first word is a whole word like any other)
+            edge[s] = ((first & 7) ? 1u << m_first : 0u) | ((lastn & 7) != 7 ? 1u << m_last : 0u);
+            inner[s] = ((2u << m_last) - (1u << m_first)) & ~edge[s];
         }
-        // every base of word m (value wv) that differs from the draft inside [first, lastn]
-        auto count_word = [&](uint32_t m, uint32_t wv) {
-            uint32_t x = wv ^ __funnelshift_r(dn32[i0 + (int)m], dn32[i0 + (int)m + 1], sh4);
-            if (m == m_first) x &= fmask;
-            if (m == m_last) x &= lmask;
-            uint32_t nz = (x | (x >> 1) | (x >> 2) | (x >> 3)) & 0x11111111u;
-            while (nz) {
-                const uint32_t t = (uint32_t)(__ffs((int)nz) - 1) >> 2;
-                nz &= nz - 1;
-                const uint32_t code = (wv >> (4 * t)) & 15u;
-                const int rel = relq + 8 * (int)m + (int)t;
-                if ((code & (code - 1)) == 0) atomicAdd(&S.sh.ex[__ffs((int)code) - 1][rel], 1u);      // A, C, G, T = 1, 2, 4, 8
-                else S.push_other(S.P0 + (uint32_t)rel, aln, 8u * m + t, 1, 1ull | ((unsigned long long)code << 4));
-            }
-        };
-        uint32_t mm = (bits & inner) | emask;
-        // the partial last word of a read that ends inside the tile is one of the two words the trim already holds: straight-line
-        if (((emask >> m_last) & 1u) && m_last - tw < 2u) {
-            mm &= ~(1u << m_last);
-            count_word(m_last, m_last == tw ? tw0 : tw1);
+    }
+    uint32_t bits = 0, cmp = 0;                                 // cmp: the whole words pass 1 compared at their own segment's offset
+#pragma unroll
+    for (int g = 0; g < TL_SEQ_QUADS; ++g) {
+        const uint32_t ga = (inner[0] >> (4 * g)) & 15u, gb = (inner[1] >> (4 * g)) & 15u;
+        if (ga | gb) {
+            const int j = (ga ? i0[0] : i0[1]) + 4 * g;
+            const uint32_t sh = ga ? sh4[0] : sh4[1];
+            const uint4 q = reinterpret_cast<const uint4*>(w)[g];
+            const uint32_t d0 = dn32[j], d1 = dn32[j + 1], d2 = dn32[j + 2], d3 = dn32[j + 3], d4 = dn32[j + 4];
+            if (q.x != __funnelshift_r(d0, d1, sh)) bits |= 1u << (4 * g);
+            if (q.y != __funnelshift_r(d1, d2, sh)) bits |= 2u << (4 * g);
+            if (q.z != __funnelshift_r(d2, d3, sh)) bits |= 4u << (4 * g);
+            if (q.w != __funnelshift_r(d3, d4, sh)) bits |= 8u << (4 * g);
+            cmp |= (ga ? ga : gb) << (4 * g);
         }
-        while (mm) {                                           // words that differ (about one word in two reads), clipped edge words
-            const uint32_t m = (uint32_t)__ffs((int)mm) - 1;
-            mm &= mm - 1;
-            count_word(m, w[m]);
+    }
+    // every base of word m (value wv) that differs from the draft inside segment s
+    auto count_word = [&](int s, uint32_t m, uint32_t wv) {
+        const int sl0 = s ? lo[1] : lo[0], sh0 = s ? hi[1] : hi[0], rq = s ? relq[1] : relq[0];
+        const int a = sl0 - 8 * (int)m, b = sh0 - 8 * (int)m;                     // the segment's nibbles of the word: [a, b)
+        if (b <= 0 || a >= 8 || b <= a) return;
+        const int j = (s ? i0[1] : i0[0]) + (int)m;
+        uint32_t x = wv ^ __funnelshift_r(dn32[j], dn32[j + 1], s ? sh4[1] : sh4[0]);
+        if (a > 0) x &= 0xFFFFFFFFu << (4 * a);
+        if (b < 8) x &= 0xFFFFFFFFu >> (32 - 4 * b);
+        uint32_t nz = (x | (x >> 1) | (x >> 2) | (x >> 3)) & 0x11111111u;
+        while (nz) {
+            const uint32_t t = (uint32_t)(__ffs((int)nz) - 1) >> 2;
+            nz &= nz - 1;
+            const uint32_t code = (wv >> (4 * t)) & 15u;
+            const int rel = rq + 8 * (int)m + (int)t;
+            if ((code & (code - 1)) == 0) atomicAdd(&S.sh.ex[__ffs((int)code) - 1][rel], 1u);      // A, C, G, T = 1, 2, 4, 8
+            else S.push_other(S.P0 + (uint32_t)rel, aln, 8u * m + t, 1, 1ull | ((unsigned long long)code << 4));
         }
     };
-    if (!one) segment((int)g0, 0, (int)nkept);
-    else if (!is_del) {
-        // aM bI cM: entry a-1 carries 1 + b bases (an "other" allele); the last run's bases sit b further along the read
-        segment((int)g0, 0, (int)ia - 1);
-        const uint8_t* pool = S.d.seq_pool;
-        S.push_other(r.gstart + ia - 1, aln, ia - 1, 1 + ib, make_sig<4>(pool, r.seq_off, len, r.flags & TR_RC, ia - 1, 1 + ib));
-        segment((int)g0 - (int)ib, (int)(ia + ib), (int)(nkept + ib));
-    } else {
-        // aM bD cM: b "-" entries, then the last run's bases sit b positions further along the reference
-        segment((int)g0, 0, (int)ia);
-        const long long t_lo = max(0ll, -(g0 + (long long)ia)), t_hi = min((long long)ib, (long long)TL_T - (g0 + (long long)ia));
-        for (long long t = t_lo; t < t_hi; ++t) atomicAdd(&S.sh.del[(int)(g0 + ia + t)], 1u);
-        segment((int)g0 + (int)ib, (int)ia, (int)nkept - (int)ib);
+    uint32_t mm = (bits & cmp) | ((inner[0] | inner[1]) & ~cmp) | edge[0] | edge[1];
+    // the partial last word of a read that ends inside the tile is one of the two words the trim already holds: straight-line (when
+    // it is not also a word of segment A before a boundary)
+    {
+        const bool sb = hi[1] > lo[1];                         // the segment that ends the read's kept entries
+        const int e_lo = sb ? lo[1] : lo[0], e_hi = sb ? hi[1] : hi[0];
+        const uint32_t m_last = (uint32_t)(e_hi - 1) >> 3;
+        if (e_hi > e_lo && (((sb ? edge[1] : edge[0]) >> m_last) & 1u) && m_last - tw < 2u && (!sb || hi[0] <= 8 * (int)m_last)) {
+            mm &= ~(1u << m_last);
+            count_word(sb ? 1 : 0, m_last, m_last == tw ? tw0 : tw1);
+        }
+    }
+    while (mm) {                                               // words that differ (about one word in two reads), edge words
+        const uint32_t m = (uint32_t)__ffs((int)mm) - 1;
+        mm &= mm - 1;
+        const uint32_t wv = w[m];
+        count_word(0, m, wv);
+        if (one) count_word(1, m, wv);
+    }
+    if (one) {
+        if (!is_del) {
+            if (ia - 1 < nkept)
+                S.push_other(r.gstart + ia - 1, aln, ia - 1, 1 + ib, make_sig<4>(S.d.seq_pool, r.seq_off, len, r.flags & TR_RC, ia - 1, 1 + ib));
+        } else {
+            const long long t0 = g0 + (long long)ia;             // the kept "-" entries: [a, min(a + b, nkept))
+            const long long t_lo = max(0ll, -t0), t_hi = min((long long)min(ib, nkept - ia), (long long)TL_T - t0);
+            for (long long t = t_lo; t < t_hi; ++t) atomicAdd(&S.sh.del[(int)(t0 + t)], 1u);
+        }
     }
     return nkept;
-}
-
-// Everything that is not the plain fast walk (queued reads, the long list, a queue that overflowed): the two-segment fast walk for
-// one-indel reads, else the general walk.  (Inlined on purpose: as an out-of-line function - half the code size - the calls cost
-// the hot loop its registers and k_tile was measured markedly slower.)
-template <int BITS>
-__device__ __forceinline__ uint32_t slow_walk(const DevData* d, TileShared* sh, uint32_t P0, TileRec r, const uint32_t* seq, uint32_t k) {
-    TileCtx<BITS> S{*d, *sh, P0};
-    uint32_t nk = NONE32;
-    if (BITS == 4 && (r.flags & TR_FAST1)) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), r, seq, k);
-    if (nk == NONE32) nk = general_walk<BITS>(S, r, k);
-    return nk;
 }
 
 // The record of sorted slot i (coalesced: consecutive lanes, consecutive 32-byte records).
@@ -1361,7 +1382,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
     if (lane == 0) { stage_bar_init(&bar[0]); stage_bar_init(&bar[1]); }
     uint32_t parity = 0;                                                       // bit s: the phase stage s completes next (kept across tiles)
     for (;;) {
-        // phase D's and the queue's generic writes to the bytes the ring shares with `wstage` come before the next tile's bulk copies:
+        // phase D's generic writes to the bytes the ring shares with `wstage` come before the next tile's bulk copies:
         // every thread fences its own writes, then the barrier
         stage_fence();
         __syncthreads();                                                       // everyone is done with the previous tile
@@ -1439,9 +1460,9 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         // so the walk starts on data that is already there.  The only gather is the 4-byte "k / contributes" word of the current
         // options, fetched one chunk ahead.
         {
-            // reads that need more than the plain fast walk (one indel: the two-segment fast walk; more indels, long reads,
-            // homopolymer tails: the general walk) go to a block-wide queue and are dealt to the warps after the chunk
-            // loop, which therefore runs the same straight-line code on every lane
+            // reads the fast walk does not take (such as two or more indels, reads longer than 192 bases, homopolymer tails of 8+ bases or
+            // longer than the last match run, reads shorter than 8, the 8-bit pool) go to a block-wide queue and are dealt to the warps
+            // after the chunk loop, which therefore runs the same straight-line code on every lane
 #ifdef PP_TILE_PROF
             unsigned long long wait_cyc = 0;
 #endif
@@ -1468,7 +1489,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                     if (k_a == 0) d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, 0u, 1u);           // adds nothing under these options
                     else {
                         uint32_t nk = NONE32;
-                        if (BITS == 4 && (rec_a.flags & (TR_FAST | TR_FAST1)) == TR_FAST) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), rec_a, seq_a, k_a);   // (one-indel reads wait for the queue: the chunk loop stays uniform)
+                        if (BITS == 4 && (rec_a.flags & TR_FAST)) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), rec_a, seq_a, k_a);
                         if (nk == NONE32) defer = true;
                         else d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, nk, k_a);
                     }
@@ -1480,7 +1501,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                         PP_PREFETCH_L2(d.cigar_ops + rec_a.cigar_off);                  // what the general walk will chase
                         PP_PREFETCH_L2(d.seq_pool + (size_t)rec_a.seq_off * (BITS == 4 ? 16 : 32));
                     } else                                                             // (a tile with more than TL_QCAP such reads)
-                        d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, slow_walk<BITS>(&d, &sh, P0, rec_a, seq_a, k_a), k_a);
+                        d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, general_walk<BITS>(S, rec_a, k_a), k_a);
                 }
                 __syncwarp();                                  // every lane is done with stage s: refill it with the chunk after next
                 if (lane == 0 && c_c < hi) issue(c_c, s);
@@ -1499,29 +1520,16 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             // the union of their paths (measured: 38 queued reads per tile took a third of the tile's time on two warps).  So the
             // queue is dealt one read per WARP first - lane 0 of every warp, then lane 1, ... - and the walks overlap instead.
             const uint32_t qn = min(sh.qn, (uint32_t)TL_QCAP);
-            // The entry carries k, and the record and the bases (which the two-segment fast walk reads from this lane's place in its
-            // warp's stage 0, free after the chunk loop) are both addressed by the slot: all of them are requested together.  (A read
-            // for the general walk has no bases in `sseq`: its 96 bytes are staged and never read.)
             for (uint32_t qi = lane * (TL_THREADS / 32) + warp; qi < qn; qi += TL_THREADS) {
-                const uint2 q = sh.queue[qi];
-                const uint32_t i = q.x, k = q.y;
-                const TileRec r = load_srec(d, i);
-                uint4* const seq = ring[0].seq + lane * TL_SEQ_QUADS;
-                if (BITS == 4) {
-                    uint4 b[TL_SEQ_QUADS];
-#pragma unroll
-                    for (int g = 0; g < TL_SEQ_QUADS; ++g) b[g] = __ldg(d.sseq + (size_t)i * TL_SEQ_QUADS + g);
-#pragma unroll
-                    for (int g = 0; g < TL_SEQ_QUADS; ++g) seq[g] = b[g];
-                }
-                d.wrec[i] = make_uint4(r.aln, r.gstart, slow_walk<BITS>(&d, &sh, P0, r, reinterpret_cast<const uint32_t*>(seq), k), k);
+                const uint2 q = sh.queue[qi];                   // (the entry carries k: the record is the only load before the walk)
+                const TileRec r = load_srec(d, q.x);
+                d.wrec[q.x] = make_uint4(r.aln, r.gstart, general_walk<BITS>(S, r, q.y), q.y);
             }
             // the long list: alignments of more than TL_LONG_E entries, looked at by every tile
             for (uint32_t i = long_lo + tid; i < long_hi; i += TL_THREADS) {
                 const TileRec r = load_srec(d, i);
                 const unsigned long long e_end = (unsigned long long)r.gstart + r.E;
                 const uint32_t k = d.kf[r.aln];
-                // (k_bin marks no long alignment TR_FAST1: the general walk is the only one they take)
                 if (k != 0 && e_end > P0 && r.gstart < P0 + (uint32_t)TL_T) d.wrec[i] = make_uint4(r.aln, r.gstart, general_walk<BITS>(S, r, k), k);
             }
         }
