@@ -115,9 +115,34 @@ static void run_shard(ShardJob* j, const pp_polish_params* prm) {
     if (j->rc != PP_OK) j->err = pp_last_error(j->ctx);
 }
 
-// Cuts a SAM file into n byte ranges for n GPUs: cut[0] = 0, cut[n] = size, every other cut is the start of a line whose QNAME differs from
-// the line before it (a read group - consecutive lines of one QNAME, alignment.rs:214-272 - is never split).  false: not a plain file,
-// or a line longer than the window (the caller lets one GPU read the whole file instead).
+// What a cut needs to know of one SAM line [p, p + len) (newline removed): 0 a blank line, an '@' line or an unaligned record (FLAG & 4),
+// which leave the open read group open; 1 an aligned record, QNAME [p, p + qlen); 2 a line whose QNAME and FLAG do not parse (the
+// tokeniser hands such a file to the host packer, so any cut will do).
+static int cut_kind(const char* p, size_t len, size_t& qlen) {
+    if (len && p[len - 1] == '\r') --len;
+    if (len == 0 || p[0] == '@') return 0;
+    const char* tab = (const char*)memchr(p, '\t', len);
+    if (!tab) return 2;
+    qlen = (size_t)(tab - p);
+    size_t i = qlen + 1, nd = 0;
+    if (i < len && p[i] == '+') ++i;
+    uint64_t v = 0;
+    for (; i < len && p[i] != '\t'; ++i, ++nd) {                       // FLAG as the tokeniser reads it (tok_line.h field_uint)
+        const unsigned d = (unsigned)(unsigned char)p[i] - '0';
+        if (d > 9) return 2;
+        v = v * 10 + d;
+        if (v > 0xFFFFFFFFull) return 2;
+    }
+    if (nd == 0 || i == len) return 2;
+    return (v & 4) ? 0 : 1;
+}
+
+// Cuts a SAM file into n byte ranges for n GPUs: cut[0] = 0, cut[n] = size, every other cut a line start that splits no read group as
+// the reference forms them (alignment.rs:238-264).  Blank lines, '@' lines and unaligned records leave the open group open, and a record
+// with an empty QNAME joins the group of the record after it, so a cut goes right before an aligned record b only when the aligned record
+// a before it has a non-empty QNAME that differs from b's (or before a line that does not parse).  Each cut moves forward from
+// g * size / n to the first such place.  false: not a plain file, or a line longer than the window (the caller lets one GPU read the
+// whole file instead).
 static bool split_ranges(const char* path, int n, std::vector<uint64_t>& cut) {
     const int fd = open(path, O_RDONLY);
     if (fd < 0) return false;
@@ -128,47 +153,61 @@ static bool split_ranges(const char* path, int n, std::vector<uint64_t>& cut) {
     cut[0] = 0;
     const size_t W = 1 << 20;
     std::vector<char> buf(W);
+    uint64_t b0 = 0, b1 = 0;                                            // buf holds bytes [b0, b1) of the file
     bool ok = true;
-    // the line starting at `pos` (a line start): its QNAME and where the next line starts
-    auto line_at = [&](uint64_t pos, std::string& qname, uint64_t& next) -> bool {
-        if (pos >= S) return false;
-        const size_t want = (size_t)std::min<uint64_t>(W, S - pos);
-        size_t got = 0;
-        while (got < want) {
-            const ssize_t r = pread(fd, buf.data() + got, want - got, (off_t)(pos + got));
-            if (r <= 0) { ok = false; return false; }
-            got += (size_t)r;
+    // the line starting at `pos` (< S): its bytes [p, p + len) and where the next line starts.  false (ok = false): a read error, or a
+    // line longer than the window
+    auto line_at = [&](uint64_t pos, const char*& p, size_t& len, uint64_t& next) -> bool {
+        for (int pass = 0; pass < 2; ++pass) {
+            if (pos >= b0 && pos < b1) {
+                const char* s = buf.data() + (pos - b0);
+                const char* nl = (const char*)memchr(s, '\n', (size_t)(b1 - pos));
+                if (nl || b1 == S) {
+                    len = nl ? (size_t)(nl - s) : (size_t)(b1 - pos);
+                    p = s;
+                    next = pos + len + 1;
+                    return true;
+                }
+            }
+            if (pass == 1) break;
+            const size_t want = (size_t)std::min<uint64_t>(W, S - pos);
+            size_t got = 0;
+            while (got < want) {
+                const ssize_t r = pread(fd, buf.data() + got, want - got, (off_t)(pos + got));
+                if (r <= 0) { ok = false; return false; }
+                got += (size_t)r;
+            }
+            b0 = pos; b1 = pos + got;
         }
-        const char* nl = (const char*)memchr(buf.data(), '\n', got);
-        if (!nl && pos + got < S) { ok = false; return false; }                  // longer than the window
-        const size_t len = nl ? (size_t)(nl - buf.data()) : got;
-        const char* tab = (const char*)memchr(buf.data(), '\t', len);
-        qname.assign(buf.data(), tab ? (size_t)(tab - buf.data()) : len);
-        next = pos + len + 1;
-        return true;
+        ok = false;
+        return false;
     };
+    const char* p = nullptr;
+    size_t len = 0, ql = 0;
+    uint64_t nx = 0;
     for (int g = 1; g < n && ok; ++g) {
         uint64_t pos = std::max<uint64_t>(S / (uint64_t)n * (uint64_t)g, cut[g - 1]);
-        if (pos >= S) { cut[g] = S; continue; }
-        // the first line start at or after pos
-        if (pos > 0) {
-            std::string q; uint64_t nx = 0;
-            if (!line_at(pos - 1, q, nx)) { if (!ok) break; cut[g] = S; continue; }       // (the rest of the line that holds byte pos - 1)
+        // the first line start at or after pos (the rest of the line that holds byte pos - 1)
+        if (pos > 0 && pos < S) {
+            if (!line_at(pos - 1, p, len, nx)) break;
             pos = std::min(nx, S);
         }
-        // ... then on to the first line whose QNAME differs from its predecessor's
-        std::string qa, qb;
-        uint64_t na = 0, nb = 0;
-        if (!line_at(pos, qa, na)) { if (!ok) break; cut[g] = S; continue; }
-        uint64_t cand = std::min(na, S);
-        for (;;) {
-            if (cand >= S || !line_at(cand, qb, nb)) { cand = S; break; }
-            if (qb != qa || (!qb.empty() && qb[0] == '@')) break;
-            qa.swap(qb);
-            cand = std::min(nb, S);
+        // ... then on to the first line a cut may go before
+        bool seen = false;                                              // an aligned record since pos, QNAME qa
+        std::string qa;
+        while (pos < S) {
+            if (!line_at(pos, p, len, nx)) break;
+            const int k = cut_kind(p, len, ql);
+            if (k == 2) break;
+            if (k == 1) {
+                if (seen && !qa.empty() && (qa.size() != ql || memcmp(qa.data(), p, ql) != 0)) break;
+                seen = true;
+                qa.assign(p, ql);
+            }
+            pos = std::min(nx, S);
         }
         if (!ok) break;
-        cut[g] = std::max(cand, cut[g - 1]);
+        cut[g] = std::max(pos, cut[g - 1]);
     }
     close(fd);
     return ok;

@@ -323,10 +323,12 @@ def test_cli_usage_errors_need_no_gpu():
 
 @pytest.mark.parametrize("seed", range(6))
 def test_sam_split_ranges_cut_between_read_groups(tmp_path, seed):
-    """pp_sam_split_ranges (multi-GPU ingestion): every cut is a line start whose QNAME differs from the previous line's."""
+    """pp_sam_split_ranges (multi-GPU ingestion): every cut is a line start, and no read group as the reference forms them
+    (tests/rangegen.py ref_groups) has aligned records on both sides of a cut."""
     import ctypes as C
     import random
     from polypolish_b200 import api
+    from tests import rangegen
     rng = random.Random(seed)
     lines = ["@HD\tVN:1.6", "@SQ\tSN:c1\tLN:1000"] if seed % 2 == 0 else []
     for r in range(rng.randint(1, 400)):
@@ -344,12 +346,8 @@ def test_sam_split_ranges_cut_between_read_groups(tmp_path, seed):
         cuts = list(cuts)
         assert cuts[0] == 0 and cuts[-1] == len(data) and cuts == sorted(cuts)
         for c in cuts[1:-1]:
-            if c == len(data):
-                continue
-            assert data[c - 1:c] == b"\n"
-            prev = data[:c - 1].rsplit(b"\n", 1)[-1].split(b"\t")[0]
-            here = data[c:].split(b"\n", 1)[0].split(b"\t")[0]
-            assert prev != here or here.startswith(b"@")
+            assert c == len(data) or data[c - 1:c] == b"\n"
+        assert rangegen.split_groups(data, cuts) == [], n
     assert L.pp_sam_split_ranges(str(tmp_path / "missing.sam").encode(), 2, (C.c_uint64 * 3)()) != 0
 
 
