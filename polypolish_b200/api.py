@@ -551,6 +551,25 @@ class Context:
         L.pp_free(out)
         return data
 
+    def filter_packed(self, m1, m2, n_names, orientation=-1, low=0.1, high=99.9):
+        """pp_filter on mate arrays (dicts of numpy arrays name_id, contig, ref_start, ref_end (uint32) and flags (uint8, bit 0 =
+        reverse)); orientation -1 = auto, 0..3 = fr, rf, ff, rr.  Returns the thresholds, orientation, pair counts and verdicts."""
+        keep, mates = [], []
+        for m in (m1, m2):
+            a = {k: np.ascontiguousarray(m[k], dtype=np.uint8 if k == "flags" else np.uint32)
+                 for k in ("name_id", "contig", "ref_start", "ref_end", "flags")}
+            keep.append(a)
+            mates.append(FilterMate(len(a["name_id"]), *(a[k].ctypes.data for k in ("name_id", "contig", "ref_start", "ref_end", "flags"))))
+        passes = [np.zeros(max(1, len(a["name_id"])), np.uint8) for a in keep]
+        res = FilterResult()
+        res.pass1, res.pass2 = passes[0].ctypes.data, passes[1].ctypes.data
+        prm = FilterParams(int(orientation), float(low), float(high), int(n_names))
+        rc = lib().pp_filter(self.h, C.byref(mates[0]), C.byref(mates[1]), C.byref(prm), C.byref(res))
+        if rc != PP_OK:
+            raise self._err(rc)
+        return dict(low=res.low, high=res.high, orientation=res.orientation, pairs=list(res.pairs), n_pass=res.n_pass,
+                    pass1=passes[0][:len(keep[0]["name_id"])], pass2=passes[1][:len(keep[1]["name_id"])], timing=res.timing.as_dict())
+
     def filter_files(self, in1, in2, out1, out2, orientation="auto", low=0.1, high=99.9, verbose=False):
         rc = lib().pp_filter_files(self.h, str(in1).encode(), str(in2).encode(), str(out1).encode(), str(out2).encode(),
                                    orientation.encode(), low, high, int(verbose))

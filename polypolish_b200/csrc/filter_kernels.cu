@@ -90,9 +90,9 @@ __global__ void __launch_bounds__(256) k_f_hist(FilterDev f, uint32_t chosen, in
     const uint32_t p0 = f.sel_prefix[0], p1 = f.sel_prefix[1];
     for (uint32_t id = blockIdx.x * blockDim.x + threadIdx.x; id < f.n_names; id += gridDim.x * blockDim.x) {
         if (f.ori[id] != chosen) continue;
-        const uint32_t v = f.ins[id], d = (v >> shift) & 255u;
-        if ((v & done_mask) == p0) atomicAdd(&s_h[0][d], 1u);
-        if ((v & done_mask) == p1) atomicAdd(&s_h[1][d], 1u);
+        const uint32_t v = f.ins[id], d = (v >> shift) & 255u, rows = filter_hist_rows(v, done_mask, p0, p1);
+        if (rows & 1u) atomicAdd(&s_h[0][d], 1u);
+        if (rows & 2u) atomicAdd(&s_h[1][d], 1u);
     }
     __syncthreads();
     if (s_h[0][threadIdx.x]) atomicAdd(&f.hist[threadIdx.x], s_h[0][threadIdx.x]);
@@ -132,17 +132,6 @@ __global__ void __launch_bounds__(256) k_f_pass(FilterDev f, int which, uint32_t
     }
     for (int o = 16; o > 0; o >>= 1) npass += __shfl_down_sync(0xffffffffu, npass, o);
     if ((threadIdx.x & 31) == 0 && npass) atomicAdd(f.n_pass + which, npass);
-}
-
-// filter.rs:249-259: rank = max(1, ceil(p / 100 * n) as usize)
-static unsigned long long nearest_rank(double percentile, unsigned long long n) {
-    const double fraction = percentile / 100.0;
-    const double r = std::ceil(fraction * (double)n);
-    unsigned long long rank;
-    if (!(r == r) || r <= 0.0) rank = 0;
-    else if (r >= 18446744073709551615.0) rank = ~0ull;
-    else rank = (unsigned long long)r;
-    return rank < 1 ? 1 : rank;
 }
 
 static unsigned grid_for(pp_ctx* ctx, size_t n) {
@@ -204,14 +193,6 @@ int filter_orientation(pp_ctx* ctx, const pp_filter_params* prm, const unsigned 
     return PP_OK;
 }
 
-void filter_ranks(const pp_filter_params* prm, unsigned long long n_sizes, unsigned long long sel_rank[2], bool in_range[2]) {
-    const unsigned long long ranks[2] = {nearest_rank(prm->low_pct, n_sizes), nearest_rank(prm->high_pct, n_sizes)};
-    for (int r = 0; r < 2; ++r) {
-        in_range[r] = ranks[r] <= n_sizes;                               // sorted_list.get(rank-1).unwrap_or(0)
-        sel_rank[r] = in_range[r] ? ranks[r] : 1;
-    }
-}
-
 int filter_hist(pp_ctx* ctx, const FilterDev& f, uint32_t chosen, int shift, uint32_t done_mask, const uint32_t prefix[2], uint32_t hist[512],
                 uint32_t* launches) {
     cudaStream_t s = pp_ctx_stream(ctx);
@@ -260,7 +241,7 @@ int pp_filter_core(pp_ctx* ctx, const Mate in[2], const pp_filter_params* prm, p
     filter_ranks(prm, n_sizes, sel_rank, in_range);
     CKF(cudaMemcpyAsync(f.sel_rank, sel_rank, 16, cudaMemcpyHostToDevice, s));
     uint32_t done_mask = 0;
-    for (int shift = 24; shift >= 0; shift -= 8) {
+    for (const int shift : FILTER_SHIFTS) {
         k_f_hist<<<grid_for(ctx, nn), 256, 0, s>>>(f, (uint32_t)chosen, shift, done_mask);
         k_f_pick<<<1, 32, 0, s>>>(f, shift);
         launches += 2;

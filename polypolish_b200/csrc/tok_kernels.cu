@@ -2217,7 +2217,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
     unsigned long long rank[2];
     filter_ranks(prm, n_sizes, rank, in_range);
     uint32_t prefix[2] = {0, 0}, done_mask = 0;
-    for (int shift = 24; shift >= 0; shift -= 8) {
+    for (const int shift : FILTER_SHIFTS) {
         rc = fx_all(S, [&](FxSide& X, int) { return filter_hist(X.ctx, X.f, (uint32_t)chosen, shift, done_mask, prefix, X.hist, &X.launches); });
         if (rc != PP_OK) return rc;
         uint32_t hist[512] = {};
