@@ -58,7 +58,8 @@ enum : unsigned {
     ERR_UNKNOWN_CONTIG = 1, ERR_SEQ_MISMATCH = 2, ERR_BAD_OP = 3, ERR_OOB = 4, ERR_NOSEQ = 5
 };
 enum : unsigned { FL_NODE_OVF = 1, FL_OUT_OVF = 8, FL_BIGGROUP = 16 };
-enum : unsigned { TR_RC = 1, TR_FAST = 2, TR_LONG = 4, TR_FAST1 = 8 };   // TR_FAST1: aM bI|bD cM, a in bits 8..15, b in 16..27, D in bit 28
+enum : unsigned { TR_RC = 1, TR_FAST = 2, TR_LONG = 4, TR_FAST1 = 8, TR_STAGED = 16 };   // TR_FAST1: aM bI|bD cM, a in bits 8..15, b in 16..27, D in bit 28
+                                                                                      // TR_STAGED: 4-bit, <= 192 bases, not long (bases in sseq)
 
 struct DevStatus {
     unsigned long long err;          // min over (aln << 8 | code); ~0 = none
@@ -95,7 +96,7 @@ struct OthNode {
 // into bin order by k_permute; everything in it is independent of the polish options.
 struct __align__(16) TileRec {
     uint32_t gstart;                 // global position of the first entry
-    uint32_t seq_off;                // PP_SEQ_BLOCK units (general walk; the fast path reads the slot's own copy of the bases)
+    uint32_t seq_off;                // PP_SEQ_BLOCK units (queued walks; the chunk loop reads a TR_STAGED slot's own copy of the bases)
     uint32_t cigar_off;
     uint32_t len_nc;                 // seq_len | n_cigar << 16
     uint32_t aln;                    // index in SAM order
@@ -103,7 +104,7 @@ struct __align__(16) TileRec {
     uint32_t flags;                  // TR_*
     uint32_t cend;                   // end of the contig (global position)
 };
-#define TL_SEQ_QUADS 6               // 16-byte quads of a slot's copy of its read (fast path: <= 192 bases)
+#define TL_SEQ_QUADS 6               // 16-byte quads of a slot's copy of its read (TR_STAGED: <= 192 bases)
 
 struct DevData {                     // everything the kernels read, by value
     // alignments
@@ -126,7 +127,7 @@ struct DevData {                     // everything the kernels read, by value
     const uint32_t* sval;            // [n_aln] alignment indices sorted by bin (stable: SAM order inside a bin)
     uint32_t* bin_start;             // [n_bins + 3] first sorted slot of every bin
     TileRec* srec;                   // [n_slots] records in slot (= bin, then SAM) order
-    uint4* sseq;                     // [n_slots * 6] 4-bit mode: every fast-path read again, forward strand, base 0 at nibble 0
+    uint4* sseq;                     // [n_slots * 6] 4-bit mode: every TR_STAGED read again, forward strand, base 0 at nibble 0
     uint32_t n_slots;                // alignments that can contribute (slots before the "nothing" key)
     const uint32_t* tile_order;      // [n_tiles] tiles by decreasing slot count: the ticket order (heavy tiles first, no long tail)
     uint32_t max_ext;                // largest entry count of a binned alignment (how many bins a tile looks back)
@@ -181,6 +182,9 @@ static inline double emu_ull2double(unsigned long long x, bool up) {
 static inline double __ull2double_rd(unsigned long long x) { return emu_ull2double(x, false); }
 static inline double __ull2double_ru(unsigned long long x) { return emu_ull2double(x, true); }
 static inline double __ull2double_rn(unsigned long long x) { return (double)x; }
+// Reads the chunk loop handed to the general walk from the pool (queued, or walked in place when the queue is full), summed over
+// the tiles that look at them: the emulator's tests read the exported symbol to see how many reads the staged walk left behind.
+inline std::atomic<unsigned long long> emu_n_queued{0};
 #endif
 
 __device__ __forceinline__ uint32_t brev4(uint32_t c) {   // complement of a BAM nibble = 4-bit reversal
@@ -222,18 +226,18 @@ template <> struct Seq<8> {
 template <int BITS> __device__ __forceinline__ bool sig_exact(unsigned long long sig) {
     return BITS == 4 ? (sig & 15ull) != 0 : (sig & 255ull) != 0;
 }
-template <int BITS>
-__device__ __forceinline__ unsigned long long make_sig(const uint8_t* pool, uint32_t off_blk, uint32_t slen, bool rc,
-                                                        uint32_t start, uint32_t len) {
+// (bs: where the read's bases are, PoolBases / StagedBases)
+template <int BITS, class Bases>
+__device__ __forceinline__ unsigned long long make_sig(const Bases& bs, uint32_t start, uint32_t len) {
     const uint32_t maxlen = BITS == 4 ? 15 : 7;
     if (len <= maxlen) {
         unsigned long long sig = len;
         for (uint32_t i = 0; i < len; ++i)
-            sig |= (unsigned long long)Seq<BITS>::read_sym(pool, off_blk, slen, rc, start + i) << ((BITS == 4 ? 4 : 8) * (i + 1));
+            sig |= (unsigned long long)bs.sym(start + i) << ((BITS == 4 ? 4 : 8) * (i + 1));
         return sig;
     }
     unsigned long long h = 0xcbf29ce484222325ull;
-    for (uint32_t i = 0; i < len; ++i) { h ^= Seq<BITS>::read_sym(pool, off_blk, slen, rc, start + i); h *= 0x100000001b3ull; }
+    for (uint32_t i = 0; i < len; ++i) { h ^= bs.sym(start + i); h *= 0x100000001b3ull; }
     h ^= len;
     return h << (BITS == 4 ? 4 : 8);
 }
@@ -400,7 +404,9 @@ __device__ __forceinline__ void bin_body(const DevData& d) {
                 const bool is_long = E > TL_LONG_E;
                 const uint32_t f0 = ops[0] & 15u;
                 const bool fast = BITS == 4 && ncig == 1 && (f0 == PP_OP_M || f0 == PP_OP_EQ) && len <= TL_FAST_LEN;
-                uint32_t flags = ((fl & PP_FLAG_RC) ? TR_RC : 0u) | (fast ? TR_FAST : 0u) | (is_long ? TR_LONG : 0u);
+                // every other short 4-bit read is walked by the general walk from its staged bases, in the chunk loop
+                const bool staged = BITS == 4 && len <= TL_FAST_LEN && !is_long;
+                uint32_t flags = ((fl & PP_FLAG_RC) ? TR_RC : 0u) | (fast ? TR_FAST : 0u) | (is_long ? TR_LONG : 0u) | (staged ? TR_STAGED : 0u);
                 if (BITS == 4 && ncig == 3 && len <= TL_FAST_LEN && !is_long) {
                     // one insertion or one deletion between two match runs: aM bI cM / aM bD cM (the fast walk hands the read to the
                     // general walk when its trim reaches past the last run)
@@ -442,7 +448,7 @@ __device__ __forceinline__ void permute_body(const DevData& d) {
     dst[0] = src[0]; dst[1] = src[1];
 }
 
-// ... and its bases (4-bit mode, fast-path reads): the EFFECTIVE read - the stored one, or its reverse complement for
+// ... and its bases (4-bit mode, TR_STAGED reads): the EFFECTIVE read - the stored one, or its reverse complement for
 // PP_FLAG_RC records (alignment.rs:161-167: complementing a BAM nibble = reversing its 4 bits, so the whole thing is one bit
 // reversal) - forward, base 0 at nibble 0, zero padded to 192 bases.  One thread per 16-byte quad (32 bases).
 __device__ __forceinline__ void permute_seq_body(const DevData& d) {
@@ -451,7 +457,7 @@ __device__ __forceinline__ void permute_seq_body(const DevData& d) {
     const uint32_t g = (uint32_t)(t % TL_SEQ_QUADS);
     if (i >= d.n_slots) return;
     const TileRec& r = d.srec[i];
-    if (!(r.flags & TR_FAST)) return;                           // the general walk reads the pool itself
+    if (!(r.flags & TR_STAGED)) return;                         // the queued general walk reads the pool itself
     const uint32_t len = r.len_nc & 0xFFFFu, nw = (len + 7) >> 3;                         // words that hold bases
     const uint32_t* s32 = reinterpret_cast<const uint32_t*>(d.seq_pool + (size_t)r.seq_off * 16);
     uint32_t out[4];
@@ -938,24 +944,52 @@ template <int BITS> struct TileCtx {
     }
 };
 
-// The general CIGAR walk of one alignment (alignment.rs:175-201, 364-378; pileup.rs:189-200), restricted to the tile.
-// Returns the number of kept entries.
-template <int BITS>
-__device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k) {
+// Where the general walk reads a read's bases, by effective read index (reverse complement applied): sym(i) = base i, read32(ri)
+// = the codes of bases [ri, ri + 32) (4-bit only; bases at indices >= len come out as garbage, the caller masks them).
+// PoolBases: the stored read in the pool, reverse complemented on the fly - the queue, the long list and the 8-bit pool.
+template <int BITS> struct PoolBases {
+    const uint8_t* p;
+    uint32_t len;
+    bool rc;
+    __device__ __forceinline__ PoolBases(const DevData& d, const TileRec& r)
+        : p(d.seq_pool + (size_t)r.seq_off * (BITS == 4 ? 16 : 32)), len(r.len_nc & 0xFFFFu), rc(r.flags & TR_RC) {}
+    __device__ __forceinline__ uint32_t sym(uint32_t i) const { return Seq<BITS>::read_sym(p, 0, len, rc, i); }
+    __device__ __forceinline__ void read32(uint32_t ri, unsigned long long& r0, unsigned long long& r1) const {
+        load_read32(reinterpret_cast<const unsigned long long*>(p), len, rc, ri, r0, r1);
+    }
+};
+// StagedBases: a TR_STAGED slot's copy in the chunk ring (k_permute_seq: forward, base i = nibble i of its 24 words).  A window
+// reads up to 4 words past the last base: the next slot's copy, or for lane 31 the first record of the stage (ChunkStage).
+struct StagedBases {
+    const uint32_t* w;
+    __device__ __forceinline__ uint32_t sym(uint32_t i) const { return (w[i >> 3] >> ((i & 7) * 4)) & 15u; }
+    __device__ __forceinline__ void read32(uint32_t ri, unsigned long long& r0, unsigned long long& r1) const {
+        const uint32_t* q = w + (ri >> 3);
+        const uint32_t sh = (ri & 7) * 4, x0 = q[0], x1 = q[1], x2 = q[2], x3 = q[3], x4 = q[4];
+        r0 = (unsigned long long)__funnelshift_r(x0, x1, sh) | (unsigned long long)__funnelshift_r(x1, x2, sh) << 32;
+        r1 = (unsigned long long)__funnelshift_r(x2, x3, sh) | (unsigned long long)__funnelshift_r(x3, x4, sh) << 32;
+    }
+};
+
+// The general CIGAR walk of one alignment (alignment.rs:175-201, 364-378; pileup.rs:189-200), restricted to the tile, reading the
+// bases from `bs`.  Returns the number of kept entries.
+template <int BITS, class Bases>
+__device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k, const Bases bs) {
     const DevData& d = S.d;
     const unsigned long long aln = r.aln;
     const uint32_t len = r.len_nc & 0xFFFFu, ncig = r.len_nc >> 16;
-    const bool rc = r.flags & TR_RC;
     const uint32_t gstart = r.gstart;
-    const uint8_t* seqp = d.seq_pool + (size_t)r.seq_off * (BITS == 4 ? 16 : 32);
     const uint32_t* ops = d.cigar_ops + r.cigar_off;
-    unsigned long long E = 0;
-    for (uint32_t p = 0; p < ncig; ++p) {
-        const uint32_t op = ops[p], o = op & 15u, l = op >> 4;
-        if (o != PP_OP_I) E += l;                               // M, =, X, D (k_prep rejected everything else)
+    unsigned long long E = r.E;                                 // (k_bin's count, exact below its saturation)
+    if (r.E == 0xFFFFFFFFu) {
+        E = 0;
+        for (uint32_t p = 0; p < ncig; ++p) {
+            const uint32_t op = ops[p], o = op & 15u, l = op >> 4;
+            if (o != PP_OP_I) E += l;                           // M, =, X, D (k_bin rejected everything else)
+        }
     }
     // trim.  Walk entries from the right; stop at the first entry that is not the single base `last`.
-    const uint32_t last = Seq<BITS>::read_sym(seqp, 0, len, rc, len - 1);
+    const uint32_t last = bs.sym(len - 1);
     unsigned long long run = 0;
     {
         uint32_t ri = len;            // read index just past the current entry's M-part
@@ -967,13 +1001,13 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k)
             if (o == PP_OP_D) {
                 // entries (ri, ri + pend): only the rightmost can carry pend; equal to `last` iff pend == 1 and base == last
                 for (uint32_t t = 0; t < l; ++t) {
-                    if (pend == 1 && Seq<BITS>::read_sym(seqp, 0, len, rc, ri) == last) { run++; pend = 0; }
+                    if (pend == 1 && bs.sym(ri) == last) { run++; pend = 0; }
                     else { stop = true; break; }
                 }
                 continue;
             }
             for (uint32_t t = 0; t < l; ++t) {                // M / = / X
-                if (pend == 0 && Seq<BITS>::read_sym(seqp, 0, len, rc, ri - 1) == last) { run++; ri--; }
+                if (pend == 0 && bs.sym(ri - 1) == last) { run++; ri--; }
                 else { stop = true; break; }
             }
         }
@@ -1002,8 +1036,8 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k)
             for (unsigned long long t = t_lo; t < t_hi; ++t) atomicAdd(&S.sh.del[(uint32_t)(gstart + e + t) - S.P0], 1u);
             if (ins && e + l - 1 < nkept) {                   // the last "-" entry absorbs a following insertion
                 const uint32_t pos = (uint32_t)(gstart + e + l - 1);
-                if (ins == 1) S.count_base(pos, Seq<BITS>::read_sym(seqp, 0, len, rc, ri), aln, ri);
-                else S.push_other(pos, aln, ri, ins, make_sig<BITS>(seqp, 0, len, rc, ri, ins));
+                if (ins == 1) S.count_base(pos, bs.sym(ri), aln, ri);
+                else S.push_other(pos, aln, ri, ins, make_sig<BITS>(bs, ri, ins));
             }
             e += l;
             continue;
@@ -1011,15 +1045,15 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k)
         if (BITS == 4) {
             for (unsigned long long c0 = t_lo & ~31ull; c0 < t_hi; c0 += 32) {
                 unsigned long long r0, r1;
-                load_read32(reinterpret_cast<const unsigned long long*>(seqp), len, rc, ri + (uint32_t)c0, r0, r1);
+                bs.read32(ri + (uint32_t)c0, r0, r1);
                 S.scan_mismatches(r0, r1, (uint32_t)min(plain64 - c0, 32ull), (uint32_t)(gstart + e + c0), aln, ri + (uint32_t)c0);
             }
         } else {
             for (unsigned long long t = t_lo; t < t_hi; ++t)
-                S.count_base((uint32_t)(gstart + e + t), Seq<BITS>::read_sym(seqp, 0, len, rc, ri + (uint32_t)t), aln, ri + (uint32_t)t);
+                S.count_base((uint32_t)(gstart + e + t), bs.sym(ri + (uint32_t)t), aln, ri + (uint32_t)t);
         }
         if (ins && e + l - 1 < nkept)
-            S.push_other((uint32_t)(gstart + e + l - 1), aln, ri + l - 1, 1 + ins, make_sig<BITS>(seqp, 0, len, rc, ri + l - 1, 1 + ins));
+            S.push_other((uint32_t)(gstart + e + l - 1), aln, ri + l - 1, 1 + ins, make_sig<BITS>(bs, ri + l - 1, 1 + ins));
         e += l;
         ri += l;
     }
@@ -1156,7 +1190,7 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, c
     if (one) {
         if (!is_del) {
             if (ia - 1 < nkept)
-                S.push_other(r.gstart + ia - 1, aln, ia - 1, 1 + ib, make_sig<4>(S.d.seq_pool, r.seq_off, len, r.flags & TR_RC, ia - 1, 1 + ib));
+                S.push_other(r.gstart + ia - 1, aln, ia - 1, 1 + ib, make_sig<4>(StagedBases{w}, ia - 1, 1 + ib));
         } else {
             const long long t0 = g0 + (long long)ia;             // the kept "-" entries: [a, min(a + b, nkept))
             const long long t_lo = max(0ll, -t0), t_hi = min((long long)min(ib, nkept - ia), (long long)TL_T - t0);
@@ -1460,9 +1494,10 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         // so the walk starts on data that is already there.  The only gather is the 4-byte "k / contributes" word of the current
         // options, fetched one chunk ahead.
         {
-            // reads the fast walk does not take (such as two or more indels, reads longer than 192 bases, homopolymer tails of 8+ bases or
-            // longer than the last match run, reads shorter than 8, the 8-bit pool) go to a block-wide queue and are dealt to the warps
-            // after the chunk loop, which therefore runs the same straight-line code on every lane
+            // a TR_STAGED read the fast walk does not take (two or more indels, X ops, homopolymer tails of 8+ bases or longer than the
+            // last match run, reads shorter than 8) is walked in place by the general walk, from its bases in the stage (only its
+            // CIGAR ops come from memory).  What is left - reads longer than 192 bases, the 8-bit pool -
+            // goes to a block-wide queue dealt to the warps after the chunk loop, each of its walks a chain of dependent loads
 #ifdef PP_TILE_PROF
             unsigned long long wait_cyc = 0;
 #endif
@@ -1490,18 +1525,23 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                     else {
                         uint32_t nk = NONE32;
                         if (BITS == 4 && (rec_a.flags & TR_FAST)) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), rec_a, seq_a, k_a);
+                        if (BITS == 4 && nk == NONE32 && (rec_a.flags & TR_STAGED))
+                            nk = general_walk<4>(reinterpret_cast<TileCtx<4>&>(S), rec_a, k_a, StagedBases{seq_a});
                         if (nk == NONE32) defer = true;
                         else d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, nk, k_a);
                     }
                 }
                 if (defer) {
+#if defined(PP_EMULATE)
+                    emu_n_queued.fetch_add(1, std::memory_order_relaxed);
+#endif
                     const uint32_t qi = atomicAdd(&sh.qn, 1u);
                     if (qi < TL_QCAP) {
                         sh.queue[qi] = make_uint2(i, k_a);
                         PP_PREFETCH_L2(d.cigar_ops + rec_a.cigar_off);                  // what the general walk will chase
                         PP_PREFETCH_L2(d.seq_pool + (size_t)rec_a.seq_off * (BITS == 4 ? 16 : 32));
                     } else                                                             // (a tile with more than TL_QCAP such reads)
-                        d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, general_walk<BITS>(S, rec_a, k_a), k_a);
+                        d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, general_walk<BITS>(S, rec_a, k_a, PoolBases<BITS>(d, rec_a)), k_a);
                 }
                 __syncwarp();                                  // every lane is done with stage s: refill it with the chunk after next
                 if (lane == 0 && c_c < hi) issue(c_c, s);
@@ -1523,14 +1563,14 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             for (uint32_t qi = lane * (TL_THREADS / 32) + warp; qi < qn; qi += TL_THREADS) {
                 const uint2 q = sh.queue[qi];                   // (the entry carries k: the record is the only load before the walk)
                 const TileRec r = load_srec(d, q.x);
-                d.wrec[q.x] = make_uint4(r.aln, r.gstart, general_walk<BITS>(S, r, q.y), q.y);
+                d.wrec[q.x] = make_uint4(r.aln, r.gstart, general_walk<BITS>(S, r, q.y, PoolBases<BITS>(d, r)), q.y);
             }
             // the long list: alignments of more than TL_LONG_E entries, looked at by every tile
             for (uint32_t i = long_lo + tid; i < long_hi; i += TL_THREADS) {
                 const TileRec r = load_srec(d, i);
                 const unsigned long long e_end = (unsigned long long)r.gstart + r.E;
                 const uint32_t k = d.kf[r.aln];
-                if (k != 0 && e_end > P0 && r.gstart < P0 + (uint32_t)TL_T) d.wrec[i] = make_uint4(r.aln, r.gstart, general_walk<BITS>(S, r, k), k);
+                if (k != 0 && e_end > P0 && r.gstart < P0 + (uint32_t)TL_T) d.wrec[i] = make_uint4(r.aln, r.gstart, general_walk<BITS>(S, r, k, PoolBases<BITS>(d, r)), k);
             }
         }
         __syncwarp();          // lanes that had a queued read rejoin their warp here: without it the warp may run phase C in two groups
