@@ -55,9 +55,10 @@ static_assert(VT_CHUNK == TL_T, "k_tile hands k_compact one chunk per tile");
 static_assert(TL_T % PP_BIN == 0 && TL_T / PP_SUB == TL_THREADS / 32 && TL_PER_THREAD * 32 == PP_SUB, "tile = whole bins; warp w owns depth sub-tile w and votes on it");
 
 enum : unsigned {
-    ERR_UNKNOWN_CONTIG = 1, ERR_SEQ_MISMATCH = 2, ERR_BAD_OP = 3, ERR_OOB = 4, ERR_NOSEQ = 5
+    ERR_UNKNOWN_CONTIG = 1, ERR_SEQ_MISMATCH = 2, ERR_BAD_OP = 3, ERR_OOB = 4, ERR_NOSEQ = 5,
+    ERR_PAST_END = 6                 // (k_bin -> k_past_end only: starts at or past its contig's end; ERR_OOB or nothing once the trim is known)
 };
-enum : unsigned { FL_NODE_OVF = 1, FL_OUT_OVF = 8, FL_BIGGROUP = 16 };
+enum : unsigned { FL_NODE_OVF = 1, FL_OUT_OVF = 8, FL_BIGGROUP = 16, FL_PAST_END = 32 };   // FL_PAST_END: k_bin left ERR_PAST_END codes
 enum : unsigned { TR_RC = 1, TR_FAST = 2, TR_LONG = 4, TR_FAST1 = 8, TR_STAGED = 16 };   // TR_FAST1: aM bI|bD cM, a in bits 8..15, b in 16..27, D in bit 28
                                                                                       // TR_STAGED: 4-bit, <= 192 bases, not long (bases in sseq)
 
@@ -373,6 +374,7 @@ __global__ void __launch_bounds__(256) k_classify_multi(DevData d) {
 template <int BITS>
 __device__ __forceinline__ void bin_body(const DevData& d) {
     uint32_t max_ext = 0;
+    bool pending = false;                                       // an alignment of this thread starts at or past its contig's end
     for (unsigned long long aln = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; aln < d.n_aln; aln += (unsigned long long)gridDim.x * blockDim.x) {
         uint32_t key = d.n_bins + 1;                            // can never contribute (k_goodk raises `err` if it is "good")
         uint32_t err = 0;
@@ -397,10 +399,14 @@ __device__ __forceinline__ void bin_body(const DevData& d) {
                 else if (o == PP_OP_D) E += l;
                 else bad = true;                                                   // alignment.rs:187-193
             }
-            if (gs >= ce) err = ERR_OOB;
-            else if (bad) err = ERR_BAD_OP;
+            // the reference checks the ops, then the length, and only then indexes the pileup - for the entries the trim keeps
+            if (bad) err = ERR_BAD_OP;
             else if (R != len) err = ERR_SEQ_MISMATCH;                             // :195-198
-            else if (!(fl & PP_FLAG_GHOST) && len != 0) {
+            else if (gs >= ce) {
+                // starts at or past the end: an overrun unless the trim removes every entry (pileup.rs:189-200).  The bases may still be
+                // on their way to the device, so k_past_end decides once they are there.
+                if (!(fl & PP_FLAG_GHOST)) { err = ERR_PAST_END; pending = true; }
+            } else if (!(fl & PP_FLAG_GHOST) && len != 0) {
                 const bool is_long = E > TL_LONG_E;
                 const uint32_t f0 = ops[0] & 15u;
                 const bool fast = BITS == 4 && ncig == 1 && (f0 == PP_OP_M || f0 == PP_OP_EQ) && len <= TL_FAST_LEN;
@@ -437,6 +443,7 @@ __device__ __forceinline__ void bin_body(const DevData& d) {
     }
     for (int o = 16; o > 0; o >>= 1) max_ext = max(max_ext, __shfl_down_sync(0xffffffffu, max_ext, o));
     if ((threadIdx.x & 31) == 0 && max_ext) atomicMax(&d.st->max_ext, max_ext);
+    if (pending) atomicOr(&d.st->flags, (unsigned)FL_PAST_END);
 }
 
 // Slot i of the binned dataset: the record of the alignment the stable sort put there.
@@ -953,6 +960,8 @@ template <int BITS> struct PoolBases {
     bool rc;
     __device__ __forceinline__ PoolBases(const DevData& d, const TileRec& r)
         : p(d.seq_pool + (size_t)r.seq_off * (BITS == 4 ? 16 : 32)), len(r.len_nc & 0xFFFFu), rc(r.flags & TR_RC) {}
+    __device__ __forceinline__ PoolBases(const DevData& d, unsigned long long aln)      // (alignment aln in SAM order)
+        : p(d.seq_pool + (size_t)d.seq_off[aln] * (BITS == 4 ? 16 : 32)), len(d.seq_len[aln]), rc(d.flags[aln] & PP_FLAG_RC) {}
     __device__ __forceinline__ uint32_t sym(uint32_t i) const { return Seq<BITS>::read_sym(p, 0, len, rc, i); }
     __device__ __forceinline__ void read32(uint32_t ri, unsigned long long& r0, unsigned long long& r1) const {
         load_read32(reinterpret_cast<const unsigned long long*>(p), len, rc, ri, r0, r1);
@@ -971,6 +980,58 @@ struct StagedBases {
     }
 };
 
+// The entries of an alignment with E entries that survive the homopolymer trim (alignment.rs:364-378): walk the entries from the
+// right, stop at the first one that is not the single base `last`, and drop that one too.  The CIGAR holds only M = X I D and
+// consumes exactly `len` >= 1 read bases.
+template <class Bases>
+__device__ __forceinline__ unsigned long long kept_entries(const uint32_t* ops, uint32_t ncig, uint32_t len, unsigned long long E, const Bases& bs) {
+    const uint32_t last = bs.sym(len - 1);
+    unsigned long long run = 0;
+    uint32_t ri = len;            // read index just past the current entry's M-part
+    uint32_t pend = 0;            // inserted bases that extend the entry being visited
+    bool stop = false;
+    for (int p = (int)ncig - 1; p >= 0 && !stop; --p) {
+        const uint32_t op = ops[p], o = op & 15u, l = op >> 4;
+        if (o == PP_OP_I) { pend += l; ri -= l; continue; }
+        if (o == PP_OP_D) {
+            // entries (ri, ri + pend): only the rightmost can carry pend; equal to `last` iff pend == 1 and base == last
+            for (uint32_t t = 0; t < l; ++t) {
+                if (pend == 1 && bs.sym(ri) == last) { run++; pend = 0; }
+                else { stop = true; break; }
+            }
+            continue;
+        }
+        for (uint32_t t = 0; t < l; ++t) {                    // M / = / X
+            if (pend == 0 && bs.sym(ri - 1) == last) { run++; ri--; }
+            else { stop = true; break; }
+        }
+    }
+    return (E - run >= 1) ? (E - run - 1) : 0;
+}
+
+// Once per dataset, after the sequence pool has arrived and only when k_bin left any ERR_PAST_END: an alignment that starts at or
+// past its contig's end is an overrun if the trim keeps an entry; if it keeps none the reference never indexes the pileup, so it
+// is a good alignment that adds nothing (k_goodk counts it in `used` and in its read group's k; its key is already "nothing").
+// The bases are the record's own or, for SEQ="*", its group's (seq_off / PP_FLAG_RC as the packers set them).
+template <int BITS>
+__device__ __forceinline__ void past_end_body(const DevData& d) {
+    for (unsigned long long aln = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; aln < d.n_aln; aln += (unsigned long long)gridDim.x * blockDim.x) {
+        const uint32_t q = d.gq[aln];
+        if (((q >> 5) & 7u) != ERR_PAST_END) continue;
+        const uint32_t ncig = d.n_cigar[aln], len = d.seq_len[aln];
+        const uint32_t* ops = d.cigar_ops + d.cigar_off[aln];
+        unsigned long long E = 0;
+        for (uint32_t p = 0; p < ncig; ++p)
+            if ((ops[p] & 15u) != PP_OP_I) E += ops[p] >> 4;  // M, =, X, D (k_bin checked the ops and the length)
+        const uint32_t err = (len != 0 && kept_entries(ops, ncig, len, E, PoolBases<BITS>(d, aln)) != 0) ? ERR_OOB : 0u;
+        d.errc[aln] = (uint8_t)err;
+        d.gq[aln] = (uint16_t)((q & ~(7u << 5)) | (err << 5));
+    }
+}
+#if !defined(PP_EMULATE)
+template <int BITS> __global__ void __launch_bounds__(256) k_past_end(DevData d) { past_end_body<BITS>(d); }
+#endif
+
 // The general CIGAR walk of one alignment (alignment.rs:175-201, 364-378; pileup.rs:189-200), restricted to the tile, reading the
 // bases from `bs`.  Returns the number of kept entries.
 template <int BITS, class Bases>
@@ -988,31 +1049,7 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k,
             if (o != PP_OP_I) E += l;                           // M, =, X, D (k_bin rejected everything else)
         }
     }
-    // trim.  Walk entries from the right; stop at the first entry that is not the single base `last`.
-    const uint32_t last = bs.sym(len - 1);
-    unsigned long long run = 0;
-    {
-        uint32_t ri = len;            // read index just past the current entry's M-part
-        uint32_t pend = 0;            // inserted bases that extend the entry being visited
-        bool stop = false;
-        for (int p = (int)ncig - 1; p >= 0 && !stop; --p) {
-            const uint32_t op = ops[p], o = op & 15u, l = op >> 4;
-            if (o == PP_OP_I) { pend += l; ri -= l; continue; }
-            if (o == PP_OP_D) {
-                // entries (ri, ri + pend): only the rightmost can carry pend; equal to `last` iff pend == 1 and base == last
-                for (uint32_t t = 0; t < l; ++t) {
-                    if (pend == 1 && bs.sym(ri) == last) { run++; pend = 0; }
-                    else { stop = true; break; }
-                }
-                continue;
-            }
-            for (uint32_t t = 0; t < l; ++t) {                // M / = / X
-                if (pend == 0 && bs.sym(ri - 1) == last) { run++; ri--; }
-                else { stop = true; break; }
-            }
-        }
-    }
-    const unsigned long long nk64 = (E - run >= 1) ? (E - run - 1) : 0;
+    const unsigned long long nk64 = kept_entries(ops, ncig, len, E, bs);
     if ((unsigned long long)gstart + nk64 > r.cend) { report_error(d.st, aln, ERR_OOB); return 0; }
     const uint32_t nkept = (uint32_t)nk64;
     S.add_interval(gstart, nkept, k);

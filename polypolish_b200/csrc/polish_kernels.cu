@@ -149,7 +149,8 @@ static void fill_data(pp_ctx* ctx, DevData& d) {
 // Once per dataset (pp_dataset_upload, pp_tok_finish): the alignments binned by position.  k_bin (record + 256-position bin key of
 // every alignment that can ever contribute) -> stable radix sort of (key, alignment) -> k_bin_bounds -> k_permute (records into
 // slot order) -> k_permute_seq (the bases of the fast-path reads into slot order, forward strand).  Nothing here depends on the
-// polish options: repeated pp_polish_resident calls reuse it, and pp_polish pays for it inside its own call.
+// polish options: repeated pp_polish_resident calls reuse it, and pp_polish pays for it inside its own call.  Alignments that start
+// at or past their contig's end wait for the bases: k_past_end trims them once seq_ready has run.
 // `seq_ready`: run right before the first kernel that reads the sequence pool (pp_dataset_upload finishes the pool's upload there).
 template <int BITS>
 static int bin_dataset(pp_ctx* ctx, const std::function<int()>& seq_ready) {
@@ -186,6 +187,7 @@ static int bin_dataset(pp_ctx* ctx, const std::function<int()>& seq_ready) {
     CK(cudaStreamSynchronize(s));
     CK(cudaGetLastError());
     ctx->max_ext = ctx->h_status->max_ext;
+    const bool past_end = ctx->h_status->flags & FL_PAST_END;
     ctx->n_slots = *h_slots;
     const size_t ns = (size_t)ctx->n_slots + 16;
     CK(ctx->b[B_SREC].ensure(ns * sizeof(TileRec)));
@@ -195,6 +197,8 @@ static int bin_dataset(pp_ctx* ctx, const std::function<int()>& seq_ready) {
     fill_data(ctx, d);
     if (ctx->n_slots) k_permute<<<(ctx->n_slots + 255) / 256, 256, 0, s>>>(d);
     if (seq_ready) { const int rc = seq_ready(); if (rc != PP_OK) return rc; }
+    if (past_end)                                               // (alignments that start at or past their contig's end: rare)
+        k_past_end<BITS><<<(uint32_t)std::min<uint64_t>((n_aln + 255) / 256, (uint64_t)ctx->sm_count * 16), 256, 0, s>>>(d);
     if (ctx->n_slots) {
         if (BITS == 4) {
             const uint64_t quads = (uint64_t)ctx->n_slots * TL_SEQ_QUADS;

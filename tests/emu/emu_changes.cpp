@@ -88,6 +88,7 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
     emu::launch((unsigned)((n_aln + 1 + 255) / 256), 256, 0, [&] { bin_bounds_body(skey.data(), (uint32_t)n_aln, n_bins + 2, bin_start.data()); });
     d.n_slots = bin_start[n_bins + 1];
     d.max_ext = st.max_ext;
+    if (st.flags & FL_PAST_END) emu::launch(2, 256, 0, [&] { past_end_body<BITS>(d); });   // (after the pool is there, as on the device)
     if (d.n_slots) {
         emu::launch((d.n_slots + 255) / 256, 256, 0, [&] { permute_body(d); });
         if (BITS == 4) emu::launch((unsigned)(((uint64_t)d.n_slots * TL_SEQ_QUADS + 255) / 256), 256, 0, [&] { permute_seq_body(d); });

@@ -84,6 +84,7 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
     emu::launch((unsigned)((n_aln + 1 + 255) / 256), 256, 0, [&] { bin_bounds_body(skey.data(), (uint32_t)n_aln, n_bins + 2, bin_start.data()); });
     d.n_slots = bin_start[n_bins + 1];
     d.max_ext = st.max_ext;
+    if (st.flags & FL_PAST_END) emu::launch(2, 256, 0, [&] { past_end_body<BITS>(d); });   // (after the pool is there, as on the device)
     g_last_max_ext = st.max_ext;
     g_last_n_long = bin_start[n_bins + 1] - bin_start[n_bins];
     g_last_bin_start.assign(bin_start.begin(), bin_start.begin() + n_bins + 2);
