@@ -59,8 +59,9 @@ enum : unsigned {
     ERR_PAST_END = 6                 // (k_bin -> k_past_end only: starts at or past its contig's end; ERR_OOB or nothing once the trim is known)
 };
 enum : unsigned { FL_NODE_OVF = 1, FL_OUT_OVF = 8, FL_BIGGROUP = 16, FL_PAST_END = 32 };   // FL_PAST_END: k_bin left ERR_PAST_END codes
-enum : unsigned { TR_RC = 1, TR_FAST = 2, TR_LONG = 4, TR_FAST1 = 8, TR_STAGED = 16 };   // TR_FAST1: aM bI|bD cM, a in bits 8..15, b in 16..27, D in bit 28
-                                                                                      // TR_STAGED: 4-bit, <= 192 bases, not long (bases in sseq)
+enum : unsigned { TR_RC = 1, TR_FAST = 2, TR_LONG = 4, TR_FAST1 = 8, TR_STAGED = 16, TR_ESC = 32 };
+// TR_FAST1: aM bI|bD cM, a in bits 8..15, b in 16..27, D in bit 28.  TR_STAGED: 4-bit, <= 192 bases, not long, every base A/C/G/T
+// (its bases in sseq).  TR_ESC: what would be TR_STAGED but has another base (N, IUPAC): walked in place from the pool
 
 struct DevStatus {
     unsigned long long err;          // min over (aln << 8 | code); ~0 = none
@@ -73,8 +74,8 @@ struct DevStatus {
     unsigned int n_changes;          // changed positions k_tile appended to the change list (counted beyond its capacity too)
     unsigned int pad1;
 #ifdef PP_TILE_PROF
-    unsigned long long prof[12];     // cycles of thread 0 per phase (A, B, queue, C, D+E), queued reads, tiles, largest queue, depth-walk cycles, walks, tiles with a walk,
-                                     // cycles lane 0 of every warp waited for its chunks' data in phase B
+    unsigned long long prof[13];     // cycles of thread 0 per phase (A, B, queue, C, D+E), queued reads, tiles, largest queue, depth-walk cycles, walks, tiles with a walk,
+                                     // cycles lane 0 of every warp waited for its chunks' data in phase B, slots the tiles scanned
 #endif
 };
 
@@ -105,7 +106,7 @@ struct __align__(16) TileRec {
     uint32_t flags;                  // TR_*
     uint32_t cend;                   // end of the contig (global position)
 };
-#define TL_SEQ_QUADS 6               // 16-byte quads of a slot's copy of its read (TR_STAGED: <= 192 bases)
+#define TL_SEQ_QUADS 3               // 16-byte quads of a slot's copy of its read (TR_STAGED: <= 192 bases, 2 bits each)
 
 struct DevData {                     // everything the kernels read, by value
     // alignments
@@ -128,7 +129,7 @@ struct DevData {                     // everything the kernels read, by value
     const uint32_t* sval;            // [n_aln] alignment indices sorted by bin (stable: SAM order inside a bin)
     uint32_t* bin_start;             // [n_bins + 3] first sorted slot of every bin
     TileRec* srec;                   // [n_slots] records in slot (= bin, then SAM) order
-    uint4* sseq;                     // [n_slots * 6] 4-bit mode: every TR_STAGED read again, forward strand, base 0 at nibble 0
+    uint4* sseq;                     // [n_slots * 3] 4-bit mode: every TR_STAGED read again as 2-bit codes, forward strand, base 0 at bits 0-1
     uint32_t n_slots;                // alignments that can contribute (slots before the "nothing" key)
     const uint32_t* tile_order;      // [n_tiles] tiles by decreasing slot count: the ticket order (heavy tiles first, no long tail)
     uint32_t max_ext;                // largest entry count of a binned alignment (how many bins a tile looks back)
@@ -456,37 +457,38 @@ __device__ __forceinline__ void permute_body(const DevData& d) {
 }
 
 // ... and its bases (4-bit mode, TR_STAGED reads): the EFFECTIVE read - the stored one, or its reverse complement for
-// PP_FLAG_RC records (alignment.rs:161-167: complementing a BAM nibble = reversing its 4 bits, so the whole thing is one bit
-// reversal) - forward, base 0 at nibble 0, zero padded to 192 bases.  One thread per 16-byte quad (32 bases).
+// PP_FLAG_RC records (alignment.rs:161-167, load_read32) - forward, as 2-bit codes A, C, G, T = 0, 1, 2, 3 with base i at bits
+// 2i, zero padded to 192 bases (48 bytes).  A read with any other base (N, IUPAC) is an escape: it becomes TR_ESC and the chunk
+// loop walks it from the pool (k_bin cannot tell: the pool arrives after the records are binned).  One thread per slot.
 __device__ __forceinline__ void permute_seq_body(const DevData& d) {
-    const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned long long i = t / TL_SEQ_QUADS;
-    const uint32_t g = (uint32_t)(t % TL_SEQ_QUADS);
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= d.n_slots) return;
-    const TileRec& r = d.srec[i];
-    if (!(r.flags & TR_STAGED)) return;                         // the queued general walk reads the pool itself
-    const uint32_t len = r.len_nc & 0xFFFFu, nw = (len + 7) >> 3;                         // words that hold bases
-    const uint32_t* s32 = reinterpret_cast<const uint32_t*>(d.seq_pool + (size_t)r.seq_off * 16);
-    uint32_t out[4];
-    if (!(r.flags & TR_RC)) {
-        const uint4 q = *reinterpret_cast<const uint4*>(s32 + 4 * g);                       // (reads past the last word stay inside the padded pool)
-        out[0] = q.x; out[1] = q.y; out[2] = q.z; out[3] = q.w;
-    } else {
-        // effective nibble e = complement of stored nibble len-1-e = nibble (8 nw - len + e) of the word-reversed, bit-reversed words
-        const uint32_t pad = 8 * nw - len;                      // 0 .. 7
-        uint32_t v[5];
+    const uint32_t flags = d.srec[i].flags;
+    if (!(flags & TR_STAGED)) return;                           // the queued general walk reads the pool itself
+    const uint32_t len = d.srec[i].len_nc & 0xFFFFu;
+    const unsigned long long* p = reinterpret_cast<const unsigned long long*>(d.seq_pool + (size_t)d.srec[i].seq_off * 16);
+    uint32_t out[4 * TL_SEQ_QUADS], esc = 0;
 #pragma unroll
-        for (int w = 0; w < 5; ++w) { const uint32_t x = 4 * g + (uint32_t)w; v[w] = x < nw ? __brev(s32[nw - 1 - x]) : 0u; }
-#pragma unroll
-        for (int w = 0; w < 4; ++w) out[w] = __funnelshift_r(v[w], v[w + 1], pad * 4);
+    for (int h = 0; h < 4 * TL_SEQ_QUADS; h += 2) {             // words h, h + 1: 32 bases per step
+        uint32_t c0 = 0, c1 = 0;
+        if (16u * (uint32_t)h < len) {
+            unsigned long long r0, r1;
+            load_read32(p, len, flags & TR_RC, 16u * (uint32_t)h, r0, r1);
+            uint32_t b0, b1;
+            c0 = pp_nib16_to_2bit(r0, b0);
+            c1 = pp_nib16_to_2bit(r1, b1);
+            const int n0 = (int)len - 16 * h, n1 = n0 - 16;                     // bases of the two words
+            const uint32_t k0 = n0 >= 16 ? 0xFFFFFFFFu : 0xFFFFFFFFu >> (32 - 2 * n0);
+            const uint32_t k1 = n1 >= 16 ? 0xFFFFFFFFu : n1 <= 0 ? 0u : 0xFFFFFFFFu >> (32 - 2 * n1);
+            c0 &= k0; c1 &= k1;                                 // nothing but zeros past the last base
+            esc |= (b0 & k0) | (b1 & k1);
+        }
+        out[h] = c0; out[h + 1] = c1;
     }
+    if (esc) { d.srec[i].flags = (flags & ~(TR_FAST | TR_FAST1 | TR_STAGED)) | TR_ESC; return; }
+    uint4* dst = d.sseq + i * TL_SEQ_QUADS;
 #pragma unroll
-    for (int w = 0; w < 4; ++w) {
-        const uint32_t m = 4 * g + (uint32_t)w;
-        if (m >= nw) out[w] = 0;
-        else if (m == nw - 1 && (len & 7)) out[w] &= 0xFFFFFFFFu >> ((8 - (len & 7)) * 4);  // nothing but zeros past the last base
-    }
-    d.sseq[t] = make_uint4(out[0], out[1], out[2], out[3]);
+    for (int g = 0; g < TL_SEQ_QUADS; ++g) dst[g] = make_uint4(out[4 * g], out[4 * g + 1], out[4 * g + 2], out[4 * g + 3]);
 }
 
 // Slots a tile has to look at (its own bins + the look-back): the weight the tiles are handed out by, heaviest first.
@@ -800,6 +802,8 @@ __device__ __forceinline__ PosOut vote_position(const OthCtx& oc, const DevParam
 #define TL_DN_HALO 32
 #define TL_INV_K 32                                  // draft nibbles are staged for tile positions [-32, T + 32)
 #define TL_DN_WORDS ((TL_T + 2 * TL_DN_HALO) / 16)
+#define TL_D2_HALO 64                                // 2-bit draft words (16 positions each) for tile positions [-64, T + 64): the
+#define TL_D2_WORDS ((TL_T + 2 * TL_D2_HALO) / 16)   // fast walk's four-word groups reach up to three words outside the tile
 
 struct WalkStage {                                     // per warp: staging of the ordered-depth merge (depth_walk_two)
     uint4 ent[64];                                     // start, kept entries, 1/k (two words)
@@ -807,10 +811,11 @@ struct WalkStage {                                     // per warp: staging of t
 };
 
 // Per warp: one chunk of the chunk loop (32 consecutive slots) in shared memory, copied in by one bulk copy per array that
-// completes on the stage's mbarrier.  Bases first: word 24 of lane 31's read, which the trim may load and then not use, is rec[0].
+// completes on the stage's mbarrier.  Bases first: words 12 and 13 of lane 31's read, which the trim and the staged general
+// walk's 32-base windows may load and then not use, are in rec[0].
 #define TL_STAGES 2
 struct ChunkStage {
-    uint4 seq[32 * TL_SEQ_QUADS];                      // 4-bit mode: the slots' bases (sseq)
+    uint4 seq[32 * TL_SEQ_QUADS];                      // 4-bit mode: the slots' bases (sseq: 48 B per slot, 2-bit codes)
     TileRec rec[32];                                   // the slots' records (srec)
 };
 
@@ -855,6 +860,9 @@ struct TileShared {
         double depth[TL_T];                            // ordered f64 depth, written over the deficit in sub-tiles that walk
     };
     unsigned long long dn[TL_DN_WORDS + 2];            // 4-bit draft codes, 16 per word, position -32 first
+    uint2 dn2[TL_D2_WORDS];                            // the fast walk's draft, 16 positions per word, position -64 first: x = 2-bit
+                                                       // A/C/G/T codes, y = 01 where the draft byte is anything else (IUPAC, N, -,
+                                                       // lower case): a read base there never matches
     union {                                            // (phase D only, behind barriers | phase B)
         WalkStage wstage[TL_THREADS / 32];             // ordered-depth merge staging, one per warp
         ChunkStage ring[TL_THREADS / 32][TL_STAGES];   // chunk-loop stages, two per warp
@@ -967,17 +975,13 @@ template <int BITS> struct PoolBases {
         load_read32(reinterpret_cast<const unsigned long long*>(p), len, rc, ri, r0, r1);
     }
 };
-// StagedBases: a TR_STAGED slot's copy in the chunk ring (k_permute_seq: forward, base i = nibble i of its 24 words).  A window
-// reads up to 4 words past the last base: the next slot's copy, or for lane 31 the first record of the stage (ChunkStage).
+// StagedBases: a TR_STAGED slot's copy in the chunk ring (k_permute_seq: forward, base i = 2-bit field i of its 12 words), handed
+// out as BAM nibbles.  A window reads up to 2 words past the last base: the next slot's copy, or for lane 31 the first record of
+// the stage (ChunkStage).
 struct StagedBases {
     const uint32_t* w;
-    __device__ __forceinline__ uint32_t sym(uint32_t i) const { return (w[i >> 3] >> ((i & 7) * 4)) & 15u; }
-    __device__ __forceinline__ void read32(uint32_t ri, unsigned long long& r0, unsigned long long& r1) const {
-        const uint32_t* q = w + (ri >> 3);
-        const uint32_t sh = (ri & 7) * 4, x0 = q[0], x1 = q[1], x2 = q[2], x3 = q[3], x4 = q[4];
-        r0 = (unsigned long long)__funnelshift_r(x0, x1, sh) | (unsigned long long)__funnelshift_r(x1, x2, sh) << 32;
-        r1 = (unsigned long long)__funnelshift_r(x2, x3, sh) | (unsigned long long)__funnelshift_r(x3, x4, sh) << 32;
-    }
+    __device__ __forceinline__ uint32_t sym(uint32_t i) const { return 1u << ((w[i >> 4] >> ((i & 15) * 2)) & 3u); }
+    __device__ __forceinline__ void read32(uint32_t ri, unsigned long long& r0, unsigned long long& r1) const { read32_2bit(w, ri, r0, r1); }
 };
 
 // The entries of an alignment with E entries that survive the homopolymer trim (alignment.rs:364-378): walk the entries from the
@@ -1098,12 +1102,13 @@ __device__ uint32_t general_walk(TileCtx<BITS>& S, const TileRec& r, uint32_t k,
 }
 
 // The fast path: a 4-bit read of at most 192 bases whose CIGAR is one M / = run, or two of them around one insertion or deletion
-// (TR_FAST1: aM bI cM / aM bD cM).  Its bases were copied into slot order when the dataset was binned - forward strand, base i =
-// nibble i (k_permute_seq) - so slot i's read is the 96 bytes at sseq + 6 i, next to its neighbours' in the tile's list: a warp's 32
-// reads are 3 KB of consecutive memory, which the chunk loop copies into shared memory with one bulk copy.  `w` = the read's 24 words
-// (shared memory; word 24 may be read and is then not used).  The draft comes from the tile's shared-memory copy through one native
-// funnel shift per 8 bases.  The read's single-base entries are at most two segments of the read, each at its own draft offset: A =
-// the first match run, B = the last one of a one-indel read (empty for a plain read).
+// (TR_FAST1: aM bI cM / aM bD cM).  Its bases were copied into slot order when the dataset was binned - forward strand, 2-bit codes,
+// base i = field i (k_permute_seq) - so slot i's read is the 48 bytes at sseq + 3 i, next to its neighbours' in the tile's list: a
+// warp's 32 reads are 1.5 KB of consecutive memory, which the chunk loop copies into shared memory with one bulk copy.  `w` = the
+// read's 12 words (shared memory; word 12 may be read and is then not used).  Every base is A/C/G/T (escapes are TR_ESC), so a
+// base differs from the draft iff its code differs from the 2-bit draft or the draft byte there is not A/C/G/T (`dn2`): one native
+// funnel shift of each per 16 bases.  The read's single-base entries are at most two segments of the read, each at its own draft
+// offset: A = the first match run, B = the last one of a one-indel read (empty for a plain read).
 //   pass 1: XOR against the draft four words at a time and only record WHICH words differ - straight-line code, no divergence.  A
 //           group of four words compares at segment A's offset if it holds a whole word of A, else at B's;
 //   pass 2: the edge words (partly outside a segment or the tile: among them the words at the boundary and those with inserted
@@ -1116,17 +1121,17 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, c
     const uint32_t len = r.len_nc & 0xFFFFu;
     const unsigned long long aln = r.aln;
     if (len < 8) return NONE32;
-    // ---- trim (alignment.rs:364-378): how many of the last bases equal the last one.  The last 8 bases as one word.
+    // ---- trim (alignment.rs:364-378): how many of the last bases equal the last one.  The last 8 bases as the low half of one word.
     uint32_t run;
-    const uint32_t tw = (len - 8) >> 3;                          // the two words the trim looks at: tw, tw + 1
+    const uint32_t tw = (len - 8) >> 4;                          // the two words the trim looks at: tw, tw + 1
     const uint32_t tw0 = w[tw], tw1 = w[tw + 1];
     {
         const uint32_t o = len - 8;
-        const uint32_t t8 = __funnelshift_r(tw0, tw1, (o & 7) * 4);
-        const uint32_t x = t8 ^ ((t8 >> 28) * 0x11111111u);
-        const uint32_t nz = (x | (x >> 1) | (x >> 2) | (x >> 3)) & 0x11111111u;
+        const uint32_t t8 = __funnelshift_r(tw0, tw1, (o & 15) * 2) & 0xFFFFu;
+        const uint32_t x = t8 ^ ((t8 >> 14) * 0x5555u);
+        const uint32_t nz = (x | (x >> 1)) & 0x5555u;
         if (nz == 0) return NONE32;                            // 8+ equal bases at the end: the general walk counts them
-        run = 7u - ((31u - (uint32_t)__clz((int)nz)) >> 2);
+        run = 7u - ((31u - (uint32_t)__clz((int)nz)) >> 1);
     }
     const bool one = r.flags & TR_FAST1;
     const uint32_t ia = (r.flags >> 8) & 0xFFu, ib = (r.flags >> 16) & 0xFFFu;            // (0 for a plain read)
@@ -1142,12 +1147,12 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, c
     S.add_interval(r.gstart, nkept, k);
     const long long g0 = (long long)r.gstart - (long long)S.P0;
     if (g0 >= (long long)TL_T || g0 + (long long)nkept <= 0) return nkept;
-    const uint32_t* dn32 = reinterpret_cast<const uint32_t*>(S.sh.dn);
+    const uint2* dn2 = S.sh.dn2;
     // Segment s: read bases [lo, hi) are single-base entries at tile-relative positions relq + base, clipped to the tile.
     //   plain: A = [0, nkept);  aM bI cM: A = [0, a - 1), entry a - 1 carries 1 + b bases (an "other" allele), B = [a + b, nkept + b) at
     //   relq - b;  aM bD cM: A = [0, a), b "-" entries, B = [a, nkept - b) at relq + b.
     int relq[2], lo[2], hi[2], i0[2];
-    uint32_t sh4[2], inner[2], edge[2];
+    uint32_t sh2[2], inner[2], edge[2];
     relq[0] = (int)g0;
     relq[1] = (int)g0 + (is_del ? (int)ib : -(int)ib);
     lo[0] = 0;
@@ -1158,15 +1163,15 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, c
     for (int s = 0; s < 2; ++s) {
         lo[s] = max(lo[s], -relq[s]);
         hi[s] = min(hi[s], (int)TL_T - relq[s]);
-        const int o0 = relq[s] + TL_DN_HALO;                   // nibble offset of word 0 in the staged draft
-        i0[s] = o0 >> 3;                                        // floor; i0 + m >= 0 for every word of a group that holds a valid word
-        sh4[s] = (uint32_t)(o0 & 7) * 4;
+        const int o0 = relq[s] + TL_D2_HALO;                   // field offset of word 0 in the staged draft
+        i0[s] = o0 >> 4;                                        // floor; i0 + m >= 1 for every word of a group that holds a valid word
+        sh2[s] = (uint32_t)(o0 & 15) * 2;
         inner[s] = edge[s] = 0;
         if (hi[s] > lo[s]) {
-            const uint32_t first = (uint32_t)lo[s], lastn = (uint32_t)(hi[s] - 1), m_first = first >> 3, m_last = lastn >> 3;
+            const uint32_t first = (uint32_t)lo[s], lastn = (uint32_t)(hi[s] - 1), m_first = first >> 4, m_last = lastn >> 4;
             // an edge word needs its own visit only when it is partly outside [first, lastn] (a read that starts inside the tile starts
             // on a word boundary: its first word is a whole word like any other)
-            edge[s] = ((first & 7) ? 1u << m_first : 0u) | ((lastn & 7) != 7 ? 1u << m_last : 0u);
+            edge[s] = ((first & 15) ? 1u << m_first : 0u) | ((lastn & 15) != 15 ? 1u << m_last : 0u);
             inner[s] = ((2u << m_last) - (1u << m_first)) & ~edge[s];
         }
     }
@@ -1176,33 +1181,31 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, c
         const uint32_t ga = (inner[0] >> (4 * g)) & 15u, gb = (inner[1] >> (4 * g)) & 15u;
         if (ga | gb) {
             const int j = (ga ? i0[0] : i0[1]) + 4 * g;
-            const uint32_t sh = ga ? sh4[0] : sh4[1];
+            const uint32_t sh = ga ? sh2[0] : sh2[1];
             const uint4 q = reinterpret_cast<const uint4*>(w)[g];
-            const uint32_t d0 = dn32[j], d1 = dn32[j + 1], d2 = dn32[j + 2], d3 = dn32[j + 3], d4 = dn32[j + 4];
-            if (q.x != __funnelshift_r(d0, d1, sh)) bits |= 1u << (4 * g);
-            if (q.y != __funnelshift_r(d1, d2, sh)) bits |= 2u << (4 * g);
-            if (q.z != __funnelshift_r(d2, d3, sh)) bits |= 4u << (4 * g);
-            if (q.w != __funnelshift_r(d3, d4, sh)) bits |= 8u << (4 * g);
+            const uint2 d0 = dn2[j], d1 = dn2[j + 1], d2 = dn2[j + 2], d3 = dn2[j + 3], d4 = dn2[j + 4];
+            if ((q.x ^ __funnelshift_r(d0.x, d1.x, sh)) | __funnelshift_r(d0.y, d1.y, sh)) bits |= 1u << (4 * g);
+            if ((q.y ^ __funnelshift_r(d1.x, d2.x, sh)) | __funnelshift_r(d1.y, d2.y, sh)) bits |= 2u << (4 * g);
+            if ((q.z ^ __funnelshift_r(d2.x, d3.x, sh)) | __funnelshift_r(d2.y, d3.y, sh)) bits |= 4u << (4 * g);
+            if ((q.w ^ __funnelshift_r(d3.x, d4.x, sh)) | __funnelshift_r(d3.y, d4.y, sh)) bits |= 8u << (4 * g);
             cmp |= (ga ? ga : gb) << (4 * g);
         }
     }
     // every base of word m (value wv) that differs from the draft inside segment s
     auto count_word = [&](int s, uint32_t m, uint32_t wv) {
         const int sl0 = s ? lo[1] : lo[0], sh0 = s ? hi[1] : hi[0], rq = s ? relq[1] : relq[0];
-        const int a = sl0 - 8 * (int)m, b = sh0 - 8 * (int)m;                     // the segment's nibbles of the word: [a, b)
-        if (b <= 0 || a >= 8 || b <= a) return;
+        const int a = sl0 - 16 * (int)m, b = sh0 - 16 * (int)m;                   // the segment's fields of the word: [a, b)
+        if (b <= 0 || a >= 16 || b <= a) return;
         const int j = (s ? i0[1] : i0[0]) + (int)m;
-        uint32_t x = wv ^ __funnelshift_r(dn32[j], dn32[j + 1], s ? sh4[1] : sh4[0]);
-        if (a > 0) x &= 0xFFFFFFFFu << (4 * a);
-        if (b < 8) x &= 0xFFFFFFFFu >> (32 - 4 * b);
-        uint32_t nz = (x | (x >> 1) | (x >> 2) | (x >> 3)) & 0x11111111u;
+        const uint32_t sh = s ? sh2[1] : sh2[0];
+        uint32_t x = (wv ^ __funnelshift_r(dn2[j].x, dn2[j + 1].x, sh)) | __funnelshift_r(dn2[j].y, dn2[j + 1].y, sh);
+        if (a > 0) x &= 0xFFFFFFFFu << (2 * a);
+        if (b < 16) x &= 0xFFFFFFFFu >> (32 - 2 * b);
+        uint32_t nz = (x | (x >> 1)) & 0x55555555u;
         while (nz) {
-            const uint32_t t = (uint32_t)(__ffs((int)nz) - 1) >> 2;
+            const uint32_t t = (uint32_t)(__ffs((int)nz) - 1) >> 1;
             nz &= nz - 1;
-            const uint32_t code = (wv >> (4 * t)) & 15u;
-            const int rel = rq + 8 * (int)m + (int)t;
-            if ((code & (code - 1)) == 0) atomicAdd(&S.sh.ex[__ffs((int)code) - 1][rel], 1u);      // A, C, G, T = 1, 2, 4, 8
-            else S.push_other(S.P0 + (uint32_t)rel, aln, 8u * m + t, 1, 1ull | ((unsigned long long)code << 4));
+            atomicAdd(&S.sh.ex[(wv >> (2 * t)) & 3u][rq + 16 * (int)m + (int)t], 1u);        // A, C, G, T = 0, 1, 2, 3
         }
     };
     uint32_t mm = (bits & cmp) | ((inner[0] | inner[1]) & ~cmp) | edge[0] | edge[1];
@@ -1211,8 +1214,8 @@ __device__ __forceinline__ uint32_t fast_walk(TileCtx<4>& S, const TileRec& r, c
     {
         const bool sb = hi[1] > lo[1];                         // the segment that ends the read's kept entries
         const int e_lo = sb ? lo[1] : lo[0], e_hi = sb ? hi[1] : hi[0];
-        const uint32_t m_last = (uint32_t)(e_hi - 1) >> 3;
-        if (e_hi > e_lo && (((sb ? edge[1] : edge[0]) >> m_last) & 1u) && m_last - tw < 2u && (!sb || hi[0] <= 8 * (int)m_last)) {
+        const uint32_t m_last = (uint32_t)(e_hi - 1) >> 4;
+        if (e_hi > e_lo && (((sb ? edge[1] : edge[0]) >> m_last) & 1u) && m_last - tw < 2u && (!sb || hi[0] <= 16 * (int)m_last)) {
             mm &= ~(1u << m_last);
             count_word(sb ? 1 : 0, m_last, m_last == tw ? tw0 : tw1);
         }
@@ -1518,6 +1521,23 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                     }
                     dn32w[wi] = v;
                 }
+                // ... and for the fast walk as 2-bit codes with the mask of the positions where no read base matches
+                for (uint32_t wi = tid; wi < TL_D2_WORDS; wi += TL_THREADS) {
+                    const long long g0 = (long long)P0 - TL_D2_HALO + 16ll * wi;
+                    unsigned long long v = 0;
+                    if (g0 >= 0 && g0 + 16 <= (long long)d.G) {
+                        const uint4 q = *reinterpret_cast<const uint4*>(d.draft + g0);       // draft is 16 B aligned, g0 a multiple of 16
+                        const uint32_t qw[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+                        for (int i = 0; i < 16; ++i) v |= (unsigned long long)asc2nib((qw[i >> 2] >> ((i & 3) * 8)) & 255u) << (4 * i);
+                    } else {
+                        for (int i = 0; i < 16; ++i)
+                            if (g0 + i >= 0 && g0 + i < (long long)d.G) v |= (unsigned long long)asc2nib(d.draft[g0 + i]) << (4 * i);
+                    }
+                    uint32_t force;
+                    const uint32_t c = pp_nib16_to_2bit(v, force);
+                    sh.dn2[wi] = make_uint2(c, force);
+                }
             }
         }
         if (c_a + lane < hi) k_a = d.kf[aln_a];                // (the SAM index has arrived while the counters were cleared)
@@ -1527,14 +1547,15 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
 #endif
         // ---- phase B: every alignment that can touch the tile: the slots of the tile's bins and of the `lb` bins before it - one
         // contiguous range of the binned dataset.  Warps take chunks of 32 consecutive slots round robin.  A chunk's records and bases
-        // are 1 KB + 3 KB of consecutive memory: lane 0 copies them into one of the warp's two stages in shared memory one chunk ahead,
+        // are 1 KB + 1.5 KB of consecutive memory: lane 0 copies them into one of the warp's two stages in shared memory one chunk ahead,
         // so the walk starts on data that is already there.  The only gather is the 4-byte "k / contributes" word of the current
         // options, fetched one chunk ahead.
         {
             // a TR_STAGED read the fast walk does not take (two or more indels, X ops, homopolymer tails of 8+ bases or longer than the
             // last match run, reads shorter than 8) is walked in place by the general walk, from its bases in the stage (only its
-            // CIGAR ops come from memory).  What is left - reads longer than 192 bases, the 8-bit pool -
-            // goes to a block-wide queue dealt to the warps after the chunk loop, each of its walks a chain of dependent loads
+            // CIGAR ops come from memory).  An escape read (TR_ESC: an N or IUPAC base) is walked in place too, from the pool.  What is
+            // left - reads longer than 192 bases, the 8-bit pool - goes to a block-wide queue dealt to the warps after the chunk loop,
+            // each of its walks a chain of dependent loads
 #ifdef PP_TILE_PROF
             unsigned long long wait_cyc = 0;
 #endif
@@ -1556,7 +1577,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 const TileRec rec_a = ring[s].rec[lane];      // (lanes past hi: bytes of an earlier chunk, not used)
                 const uint32_t* const seq_a = reinterpret_cast<const uint32_t*>(ring[s].seq + lane * TL_SEQ_QUADS);
                 const uint32_t i = c_a + lane;
-                bool defer = false;
+                bool defer = false, esc = false;
                 if (i < hi) {
                     if (k_a == 0) d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, 0u, 1u);           // adds nothing under these options
                     else {
@@ -1564,20 +1585,23 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                         if (BITS == 4 && (rec_a.flags & TR_FAST)) nk = fast_walk(reinterpret_cast<TileCtx<4>&>(S), rec_a, seq_a, k_a);
                         if (BITS == 4 && nk == NONE32 && (rec_a.flags & TR_STAGED))
                             nk = general_walk<4>(reinterpret_cast<TileCtx<4>&>(S), rec_a, k_a, StagedBases{seq_a});
-                        if (nk == NONE32) defer = true;
+                        if (nk == NONE32) { defer = true; esc = BITS == 4 && (rec_a.flags & TR_ESC); }
                         else d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, nk, k_a);
                     }
                 }
                 if (defer) {
+                    uint32_t qi = TL_QCAP;                     // an escape read is walked right here
+                    if (!esc) {
 #if defined(PP_EMULATE)
-                    emu_n_queued.fetch_add(1, std::memory_order_relaxed);
+                        emu_n_queued.fetch_add(1, std::memory_order_relaxed);
 #endif
-                    const uint32_t qi = atomicAdd(&sh.qn, 1u);
+                        qi = atomicAdd(&sh.qn, 1u);
+                    }
                     if (qi < TL_QCAP) {
                         sh.queue[qi] = make_uint2(i, k_a);
                         PP_PREFETCH_L2(d.cigar_ops + rec_a.cigar_off);                  // what the general walk will chase
                         PP_PREFETCH_L2(d.seq_pool + (size_t)rec_a.seq_off * (BITS == 4 ? 16 : 32));
-                    } else                                                             // (a tile with more than TL_QCAP such reads)
+                    } else                                                             // (or a tile with more than TL_QCAP queued reads)
                         d.wrec[i] = make_uint4(rec_a.aln, rec_a.gstart, general_walk<BITS>(S, rec_a, k_a, PoolBases<BITS>(d, rec_a)), k_a);
                 }
                 __syncwarp();                                  // every lane is done with stage s: refill it with the chunk after next
@@ -1586,6 +1610,7 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             }
 #ifdef PP_TILE_PROF
             if (lane == 0 && wait_cyc) atomicAdd(&d.st->prof[11], wait_cyc);
+            if (tid == 0) atomicAdd(&d.st->prof[12], (unsigned long long)(hi - lo));
 #endif
         }
         __syncthreads();

@@ -201,8 +201,7 @@ static int bin_dataset(pp_ctx* ctx, const std::function<int()>& seq_ready) {
         k_past_end<BITS><<<(uint32_t)std::min<uint64_t>((n_aln + 255) / 256, (uint64_t)ctx->sm_count * 16), 256, 0, s>>>(d);
     if (ctx->n_slots) {
         if (BITS == 4) {
-            const uint64_t quads = (uint64_t)ctx->n_slots * TL_SEQ_QUADS;
-            k_permute_seq<<<(uint32_t)((quads + 255) / 256), 256, 0, s>>>(d);
+            k_permute_seq<<<(ctx->n_slots + 255) / 256, 256, 0, s>>>(d);
         }
     }
     {   // tiles by decreasing slot count (the persistent kernel hands them out in that order)
@@ -492,6 +491,12 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
                 (double)hs.prof[4] / hs.prof[6], (double)hs.prof[5] / hs.prof[6], hs.prof[7], (double)hs.prof[11] / hs.prof[6] / (TL_THREADS / 32));
         fprintf(stderr, "[tile prof] depth walks %llu (%.2f per tile, %llu tiles with one), %.0f cycles each\n", hs.prof[9], (double)hs.prof[9] / hs.prof[6], hs.prof[10],
                 hs.prof[9] ? (double)hs.prof[8] / hs.prof[9] : 0.0);
+        {   // what the chunk loop streams per call, by array, from the slots the tiles scanned (look-back bins included)
+            const double sl = (double)hs.prof[12], t = (double)hs.prof[6];
+            fprintf(stderr, "[tile prof] slots scanned %llu; MB: records %.1f bases %.1f kf %.1f wrec %.1f draft+verdicts+chain heads %.1f\n",
+                    hs.prof[12], sl * sizeof(TileRec) / 1e6, BITS == 4 ? sl * 16 * TL_SEQ_QUADS / 1e6 : 0.0, sl * 4 / 1e6, sl * 16 / 1e6,
+                    t * (TL_T + 16 + 2 * TL_T + 4 * TL_T) / 1e6);
+        }
 #endif
         if (hs.err != ~0ull) {
             res->error_aln = (int64_t)(hs.err >> 8);
