@@ -160,7 +160,12 @@ int pp_polish(pp_ctx* ctx, const pp_contigs* contigs, const pp_alignments* alns,
               const pp_polish_params* params, pp_polish_result* result);
 
 /* Device-resident variant (kernel-path timing; repeated polishing with different options):
- * upload once, polish many times, fetch when wanted. */
+ * upload once, polish many times, fetch when wanted.  Every option may differ from call to call, --careful included: which
+ * records are good, k and --careful are decided per call, as process_one_read does (alignment.rs:275-305).  The one thing the
+ * load decides is what happens to a read group of several records none of which has a SEQ: a load without --careful refuses it
+ * (pp_pack_create, pp_tok_begin), a load with --careful keeps it (PP_FLAG_NOSEQ), and then a call without --careful fails with
+ * PP_ERR_INPUT "no alignments for read contain sequence (alignment i)", i = the group's first record, whether or not any of its
+ * records is good; an earlier group's error still comes first, as in the reference. */
 int pp_dataset_upload(pp_ctx* ctx, const pp_contigs* contigs, const pp_alignments* alns);
 int pp_polish_resident(pp_ctx* ctx, const pp_polish_params* params, pp_polish_result* result);
 
@@ -256,6 +261,9 @@ typedef struct pp_pack pp_pack;
 /* SAM text -> pp_alignments.  Restates the text side of add_to_pileup (alignment.rs:225-272) and
  * Alignment::new (alignment.rs:49-98): line skipping, column checks, NM / ZP tags, CIGAR validation,
  * QNAME grouping, source sequence of SEQ="*" records. */
+/* careful: the --careful of the load.  Without it, a read group of several records none of which has a SEQ fails the file with the
+ * reference's "no alignments for read <QNAME> contain sequence"; with it, the group is kept (its records PP_FLAG_NOSEQ) and every
+ * polish call without --careful fails on it (pp_polish_resident). */
 pp_pack* pp_pack_create(const pp_fasta* f, int careful);
 void pp_pack_free(pp_pack* p);
 int pp_pack_add_sam_file(pp_pack* p, const char* path);                        /* PP_OK / PP_ERR_INPUT / PP_ERR_IO */
@@ -297,6 +305,8 @@ typedef struct {
   uint32_t launches;
   uint64_t h2d_bytes;                  /* bytes that crossed PCIe for this file (less than its size when QUAL was dropped) */
 } pp_tok_stats;
+/* careful: as pp_pack_create's.  Without it a read group of several records without any SEQ returns PP_TOK_HOST (the host packer
+ * then raises the reference's error); with it the group is kept and a later pp_polish_resident without --careful fails on it. */
 int pp_tok_begin(pp_ctx* ctx, const pp_fasta* assembly, int careful, int seq_bits /* 4 | 8 */);
 int pp_tok_add_text(pp_ctx* ctx, const char* text, size_t len, pp_tok_stats* stats /* may be NULL */);
 int pp_tok_add_file(pp_ctx* ctx, const char* path, pp_tok_stats* stats /* may be NULL */);

@@ -382,8 +382,8 @@ __device__ __forceinline__ void bin_body(const DevData& d) {
         const uint32_t c = d.contig[aln];
         const uint8_t fl = d.flags[aln];
         const uint32_t ncig = d.n_cigar[aln], cigoff = d.cigar_off[aln];
-        if (c == PP_CONTIG_UNKNOWN) err = ERR_UNKNOWN_CONTIG;                      // alignment.rs:298-300
-        else if (fl & PP_FLAG_NOSEQ) err = ERR_NOSEQ;
+        if (fl & PP_FLAG_NOSEQ) err = ERR_NOSEQ;                                    // before anything else (alignment.rs:280-281)
+        else if (c == PP_CONTIG_UNKNOWN) err = ERR_UNKNOWN_CONTIG;                 // alignment.rs:298-300
         else if (ncig == 0) err = ERR_BAD_OP;                                      // the packer never emits this
         else {
             const unsigned long long gs = d.contig_off[c] + d.ref_start[aln];
@@ -568,9 +568,13 @@ __device__ __forceinline__ void goodk_body(const DevData& d, PrepShared& sh) {
         }
         if (q & GQ_GHOST) good = false;                         // another shard scatters it; it only counted towards k
         uint32_t kf = 0;
+        const uint32_t e = (q >> 5) & 7u;                       // what the reference raises for a good alignment (found once, by k_bin)
+        // ... except "no sequence", which the reference raises for the whole group before goodness is looked at, unless --careful
+        // skips the group (alignment.rs:277-281).  Only a load with --careful keeps such a group (PP_FLAG_NOSEQ), and every one of
+        // its records carries the error, so the group's first record is the one named.
+        if (e == ERR_NOSEQ && !prm.careful) report_error(d.st, aln, e);
         if (good) {
             used++;
-            const uint32_t e = (q >> 5) & 7u;                   // what the reference raises for a good alignment (found once, by k_bin)
             if (e) report_error(d.st, aln, e);
             else kf = k;
         }

@@ -299,21 +299,103 @@ def expect_global_k(read_id, good):
     return False
 
 
-def record_good(sam_texts, max_errors=10, careful=False, **_):
-    """alignment.rs goodness of every aligned record, in SAM order (the records these generators write: NM tag, M ends, ZP:Z:fail).
-    --careful drops every record of a multi-record group."""
-    rows = [l.split("\t") for t in sam_texts for l in t.split("\n") if l and not l.startswith("@")]
-    good = []
-    for i, r in enumerate(rows):
-        nm = int([x for x in r[11:] if x.startswith("NM:i:")][0][5:])
-        ops = re.findall(r"\d+([MIDNSHP=X])", r[5])
-        ends = ops[0] in "M=" and ops[-1] in "M="
-        g = ends and nm <= max_errors and "ZP:Z:fail" not in r[11:]
-        if careful:
-            multi = (i > 0 and rows[i - 1][0] == r[0]) or (i + 1 < len(rows) and rows[i + 1][0] == r[0])
-            g = g and not multi
-        good.append(g)
-    return good
+_COMP = str.maketrans("ACGTacgt", "TGCAtgca")
+
+
+def _kept_entries(cigar, seq):
+    """Entries of an alignment after the homopolymer trim (alignment.rs:175-201, 364-378), or the error its walk raises first:
+    "bad_op" (an op other than M = X I D), "seq_mismatch" (read bases consumed != len(SEQ))."""
+    entries, i = [], 0
+    for n, op in re.findall(r"(\d+)([MIDNSHP=X])", cigar):
+        for _ in range(int(n)):
+            if op in "M=X":
+                entries.append((i, i + 1))
+                i += 1
+            elif op == "I":
+                entries[-1] = (entries[-1][0], i + 1)
+                i += 1
+            elif op == "D":
+                entries.append((i, i))
+            else:
+                return "bad_op"
+    if i != len(seq):
+        return "seq_mismatch"
+    last = seq[entries[-1][0]:entries[-1][1]]
+    while entries and seq[entries[-1][0]:entries[-1][1]] == last:
+        entries.pop()
+    return max(0, len(entries) - 1)
+
+
+def record_good(sam_texts, max_errors=10, careful=False, contigs=None, detail=False, **_):
+    """process_one_read (alignment.rs:240-305) on SAM texts in file order.  Without `detail`: the goodness of every aligned record, in
+    SAM order.  With it: dict(good, k = good records per group, groups = (first alignment, size) per group, used = the reference's
+    used_total, error = the first error the reference raises as (kind, alignment index) or None), where `contigs` maps contig names
+    to lengths.  Unaligned records (flag 4) are skipped and neither end nor join a group; a group ends at a QNAME change or at the end
+    of its file, and a record after an empty QNAME joins that group (:255).  --careful skips every group of more than one record
+    (:277-279); a group none of whose records has SEQ raises "noseq" on its first record (:280), before goodness; a record is good
+    if its expanded CIGAR starts and ends with M / =, NM <= max_errors and no tag equals ZP:Z:fail ignoring case (:59-78, :151-155,
+    :283-287).  Then each good record in order may raise "unknown_contig" (:298-300), "bad_op", "seq_mismatch" or "oob" (an entry
+    kept by the trim past its contig's end, pileup.rs:189-200).  Kinds: emu_lib.ERR_TEXT codes by name (ERR_KIND)."""
+    groups = []
+    n = 0
+    for t in sam_texts:
+        name, cur = "", []
+        for line in t.split("\n"):
+            if not line or line.startswith("@"):
+                continue
+            r = line.split("\t")
+            if int(r[1]) & 4:
+                continue
+            if name == "" or name == r[0]:
+                cur.append((n, r))
+            else:
+                groups.append(cur)
+                cur = [(n, r)]
+            name = r[0]
+            n += 1
+        if cur:
+            groups.append(cur)
+    good = [False] * n
+    ks, bounds, used, error = [], [], 0, None
+    for grp in groups:
+        bounds.append((grp[0][0], len(grp)))
+        if careful and len(grp) > 1:
+            ks.append(0)
+            continue
+        src = next((r for _, r in grp if r[9] != "*"), None)
+        if src is None:
+            error = error or ("noseq", grp[0][0])
+            ks.append(0)
+            continue
+        gs = []
+        for i, r in grp:
+            nm = [int(x[5:]) for x in r[11:] if x.startswith("NM:i:")][-1]
+            ops = re.findall(r"\d+([MIDNSHP=X])", r[5])
+            if ops[0] in "M=" and ops[-1] in "M=" and nm <= max_errors and not any(x.lower() == "zp:z:fail" for x in r[11:]):
+                good[i] = True
+                gs.append((i, r))
+        ks.append(len(gs))
+        used += len(gs)
+        for i, r in gs:
+            if error or contigs is None:
+                break
+            if r[2] not in contigs:
+                error = ("unknown_contig", i)
+                break
+            seq = r[9]
+            if seq == "*":
+                seq = src[9] if (int(r[1]) & 16) == (int(src[1]) & 16) else src[9][::-1].translate(_COMP)
+            kept = _kept_entries(r[5], seq)
+            if isinstance(kept, str):
+                error = (kept, i)
+            elif max(int(r[3]) - 1, 0) + kept > contigs[r[2]]:
+                error = ("oob", i)
+    if not detail:
+        return good
+    return dict(good=good, k=ks, groups=bounds, used=used, error=error)
+
+
+ERR_KIND = {"unknown_contig": 1, "seq_mismatch": 2, "bad_op": 3, "oob": 4, "noseq": 5}
 
 
 # ---- E. depth on a vote boundary -------------------------------------------------------------------------------------------
