@@ -212,6 +212,20 @@ int pp_polish_changes_fetch(pp_ctx* ctx, uint64_t row_cap, uint64_t* pos, pp_deb
  * in the assembly's contig order and position order.  NULL or "" switches it off (the default).  The path is copied. */
 int pp_set_changes_file(pp_ctx* ctx, const char* path);
 
+/* The status runs (--status-bed): every position's BaseStatus (pileup.rs:18-25, 114-129; the --debug status column) as runs of
+ * equal status.  Recording is off by default; like pp_polish_set_changes it keeps the vote's shortcuts, and it costs one byte per
+ * position on the device while it is on.  Switch it on before the polish call (1 record, 2 stop but keep the last runs, 0 off). */
+int pp_polish_set_status(pp_ctx* ctx, int on);
+/* runs of the last polish with recording on, in position order: start[i] = global position, status[i] = 0..5 as
+ * pp_debug_pos.status; run i ends at start[i + 1] (or at total bp); every contig start begins a run.  Call once with
+ * run_cap = 0 for *n_runs. */
+int pp_polish_status_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint8_t* status, uint64_t* n_runs);
+/* The whole-command calls below (pp_polish_files, pp_polish_files_multi, pp_filter_polish_files, pp_filter_polish_files_multi) made
+ * with `ctx` (ctxs[0]) as their context also write the status runs to `path` as BED: "<contig>\t<start>\t<end>\t<status>\n" per
+ * run, 0-based half-open, contigs in the assembly's order, no header.  NULL or "" switches it off (the default).  The path is
+ * copied. */
+int pp_set_status_file(pp_ctx* ctx, const char* path);
+
 /* ------------------------------------------------------------------------------------------------------
  * filter (filter.rs).  One record per ALIGNED line of one mate's SAM file, in file order.
  * Replaces get_insert_size_thresholds (filter.rs:148-186) and alignment_pass_qc (filter.rs:352-377).

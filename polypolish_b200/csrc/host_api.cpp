@@ -225,7 +225,7 @@ using FastaPtr = std::unique_ptr<pp_fasta, Deleter<pp_fasta_free>>;
 using PackPtr = std::unique_ptr<pp_pack, Deleter<pp_pack_free>>;
 using ShardsPtr = std::unique_ptr<pp_shards, Deleter<pp_shards_free>>;
 
-// --debug / --changes: the contexts record per-position data (Set = pp_polish_set_debug / pp_polish_set_changes) for the length of
+// --debug / --changes / --status-bed: the contexts record per-position data (Set = pp_polish_set_debug / pp_polish_set_changes / pp_polish_set_status) for the length of
 // the call.  They are left in mode 2 (not recording, the records of this call readable) when the call succeeded, otherwise in mode
 // 0, so that later calls neither record nor read stale data.
 template <int (*Set)(pp_ctx*, int)>
@@ -540,6 +540,12 @@ static std::string assemble(const pp_fasta* fa, const pp_contigs& contigs, const
     return out;
 }
 
+// A global position of job j's own assembly -> (input contig, position in that contig).
+static std::pair<uint32_t, uint64_t> input_position(const ShardJob& j, bool one_job, uint64_t pos) {
+    const uint32_t lc = (uint32_t)(std::upper_bound(j.contigs.off, j.contigs.off + j.contigs.n_contigs + 1, pos) - j.contigs.off) - 1;
+    return {one_job ? lc : j.contig_map[lc], pos - j.contigs.off[lc]};
+}
+
 // --changes: the --debug rows of the changed positions, in the input FASTA's contig order, then position order.  Every job reports
 // the rows of its own contigs (pp_polish_changes_fetch); they are merged here.  PP_ERR_IO: the file could not be written; another
 // error: its message is on ctx.
@@ -558,9 +564,9 @@ static int write_changes(pp_ctx* ctx, const pp_fasta* fa, const std::vector<Shar
             rc = pp_polish_changes_fetch(j.ctx, n, g.pos.data(), g.rows.data(), g.off.data(), g.pool.data(), bytes, &n, &bytes);
         }
         if (rc != PP_OK) return pp_ctx_fail(ctx, rc, std::string(pp_last_error(j.ctx)).c_str());
-        for (uint64_t i = 0; i < n; ++i) {             // global position in the job's own assembly -> (input contig, position in it)
-            const uint32_t lc = (uint32_t)(std::upper_bound(j.contigs.off, j.contigs.off + j.contigs.n_contigs + 1, g.pos[i]) - j.contigs.off) - 1;
-            order.push_back({jobs.size() == 1 ? lc : j.contig_map[lc], g.pos[i] - j.contigs.off[lc], s, i});
+        for (uint64_t i = 0; i < n; ++i) {
+            const auto cp = input_position(j, jobs.size() == 1, g.pos[i]);
+            order.push_back({cp.first, cp.second, s, i});
         }
     }
     std::sort(order.begin(), order.end(), [](const Row& a, const Row& b) { return a.contig != b.contig ? a.contig < b.contig : a.pos < b.pos; });
@@ -569,6 +575,39 @@ static int write_changes(pp_ctx* ctx, const pp_fasta* fa, const std::vector<Shar
     for (const Row& r : order) {
         const Fetched& g = got[r.job];
         rows.add(buf, pp_fasta_name(fa, r.contig), r.pos, g.rows[r.i], g.pool.data() + g.off[r.i]);
+    }
+    return fwrite(buf.data(), 1, buf.size(), f) == buf.size() ? PP_OK : PP_ERR_IO;
+}
+
+// --status-bed: the status runs as BED lines, contigs in the input FASTA's order.  Every job reports the runs of its own contigs
+// (pp_polish_status_fetch); a run never crosses a contig, so each contig's lines are its runs in order.  PP_ERR_IO: the file could not
+// be written; another error: its message is on ctx.
+static int write_status_bed(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>& jobs, FILE* f) {
+    static const char* const word[6] = {"low_depth", "none", "multiple", "too_close", "kept", "changed"};
+    struct Run { uint64_t start, end; uint8_t status; };
+    std::vector<std::vector<Run>> by_contig(contigs.n_contigs);
+    for (const ShardJob& j : jobs) {
+        uint64_t n = 0;
+        int rc = pp_polish_status_fetch(j.ctx, 0, nullptr, nullptr, &n);
+        std::vector<uint64_t> start(n);
+        std::vector<uint8_t> status(n);
+        if (rc == PP_OK && n) rc = pp_polish_status_fetch(j.ctx, n, start.data(), status.data(), &n);
+        if (rc != PP_OK) return pp_ctx_fail(ctx, rc, std::string(pp_last_error(j.ctx)).c_str());
+        const uint64_t G = j.contigs.off[j.contigs.n_contigs];
+        for (uint64_t i = 0; i < n; ++i) {
+            const auto cp = input_position(j, jobs.size() == 1, start[i]);
+            const uint64_t end = i + 1 < n ? start[i + 1] : G;
+            by_contig[cp.first].push_back({cp.second, cp.second + (end - start[i]), status[i]});
+        }
+    }
+    std::string buf;
+    char tmp[64];
+    for (uint32_t c = 0; c < contigs.n_contigs; ++c) {
+        const char* name = pp_fasta_name(fa, c);
+        for (const Run& r : by_contig[c]) {
+            snprintf(tmp, sizeof tmp, "\t%llu\t%llu\t", (unsigned long long)r.start, (unsigned long long)r.end);
+            buf += name; buf += tmp; buf += word[r.status < 6 ? r.status : 0]; buf += '\n';
+        }
     }
     return fwrite(buf.data(), 1, buf.size(), f) == buf.size() ? PP_OK : PP_ERR_IO;
 }
@@ -614,9 +653,21 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
         changes_file = fopen(changes_path.c_str(), "wb");
         if (!changes_file) { if (debug_file) fclose(debug_file); return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + changes_path + "\"").c_str()); }
     }
-    struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file}, closer2{changes_file};
+    const std::string status_path = pp_ctx_status_file(ctx);
+    const bool status = !status_path.empty();
+    FILE* status_file = nullptr;
+    if (status) {
+        status_file = fopen(status_path.c_str(), "wb");
+        if (!status_file) {
+            if (debug_file) fclose(debug_file);
+            if (changes_file) fclose(changes_file);
+            return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + status_path + "\"").c_str());
+        }
+    }
+    struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file}, closer2{changes_file}, closer3{status_file};
     Recording<pp_polish_set_debug> recording(&ctx, 1, debug);
     Recording<pp_polish_set_changes> recording_changes(ctxs, n_ctx, changes);
+    Recording<pp_polish_set_status> recording_status(ctxs, n_ctx, status);
 
     // the first SAM file starts streaming into HBM while the assembly is loaded
     const bool device_parser = pp_get_parser(ctx) == 0;
@@ -669,8 +720,12 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
         rc = write_changes(ctx, fa.get(), ld.jobs, changes_file);
         if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + changes_path + "\"").c_str());
     }
+    if (rc == PP_OK && status) {
+        rc = write_status_bed(ctx, fa.get(), contigs, ld.jobs, status_file);
+        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + status_path + "\"").c_str());
+    }
     if (rc != PP_OK) return rc;
-    recording.ok = recording_changes.ok = true;
+    recording.ok = recording_changes.ok = recording_status.ok = true;
     if (verbose) {
         uint64_t n_used = 0;
         for (const ShardJob& j : ld.jobs) n_used += j.res.n_aln_used;

@@ -695,6 +695,9 @@ struct VoteParams {
     uint32_t* chg_pos;                // [chg_cap] global position of each record
     unsigned int* chg_n;              // records appended (DevStatus::n_changes); more than chg_cap: the list overflowed
     uint32_t chg_cap;
+    // --status-bed: one byte per position (padded to whole SR_CHUNKs), bits 0..2 the BaseStatus as pp_debug_pos.status, bit 7 set where
+    // a contig starts; k_status_runs turns it into runs.  Read only by k_tile's status mode.
+    uint8_t* sts;
 };
 
 // What the other-allele slow path needs, passed by value so that the kernel parameter structs are never
@@ -1438,10 +1441,10 @@ __device__ __forceinline__ void depth_walk(const DevData& d, TileShared& sh, Wal
     } else depth_walk_steps<BITS>(d, sh, P0, sub, lb, long_lo, long_hi);
 }
 
-// CHG: the change report is recorded (vp.chg; without it the vp.chg* fields are not read).  A template argument, so that the kernel
-// without the report does the work it did before the report existed (as a run-time test it measured up to 0.5 % slower on an H100,
-// 700 W, 5 Mbp x 100x).
-template <int BITS, bool CHG = false>
+// CHG: the change report is recorded (vp.chg; without it the vp.chg* fields are not read).  STS: every position's status is
+// recorded (vp.sts).  Template arguments, so that the kernel without a report does the work it did before the reports existed (as a
+// run-time test CHG measured up to 0.5 % slower on an H100, 700 W, 5 Mbp x 100x).
+template <int BITS, bool CHG = false, bool STS = false>
 __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp, TileShared& sh) {
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const DevParams prm = *d.prm;
@@ -1676,6 +1679,8 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         // threshold (the same tests as in phase E, on the lower bound), else when both ends of the bound give the same thresholds.
         // The debug records print depth itself: there every sub-tile with k != 1 coverage walks.  The change records print it too:
         // there a sub-tile also walks when one of its positions passes these tests, which every position that reaches the vote does.
+        // The status reads depth only through the thresholds (vote_thresholds): in status mode a sub-tile also walks when a position
+        // with k != 1 coverage gets other thresholds at the two ends of its bound, whatever the tests say of the emitted base.
         bool walk;
         {
             bool open = false;
@@ -1685,6 +1690,10 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                     if (!((multi >> i) & 1u)) continue;
                     const uint32_t rel = rel0 + i;
                     if (cover[i] >= TL_DEF_COVER) { open = true; continue; }
+                    if (STS) {
+                        const DepthBounds db = depth_bounds(cover[i], sh.deficit[rel]);
+                        if (!same_thresholds(prm, db.lo, db.hi)) { open = true; continue; }
+                    }
                     const uint32_t mx = max(max(max(sh.ex[0][rel], sh.ex[1][rel]), max(sh.ex[2][rel], sh.ex[3][rel])), max(sh.del[rel], sh.oth[rel]));
                     if (mx == 0 || mx < prm.min_depth) continue;
                     const DepthBounds db = depth_bounds(cover[i], sh.deficit[rel]);
@@ -1715,6 +1724,8 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             ctg = clo;
         }
         uint32_t next_start = (ctg + 1 < d.n_contigs) ? (uint32_t)d.contig_off[ctg + 1] : 0xFFFFFFFFu;
+        uint32_t sts4 = 0, ctg_start = 0;                  // status mode: the four status bytes; the start of contig ctg
+        if constexpr (STS) ctg_start = (p0 < d.G) ? (uint32_t)d.contig_off[ctg] : 0u;
         const uint32_t dr = *reinterpret_cast<const uint32_t*>(d.draft + p0);      // draft is padded past G
 #pragma unroll
         for (int i = 0; i < TL_PER_THREAD; ++i) {
@@ -1728,14 +1739,17 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 n_changed = n_zero = 0;
                 tdepth = 0.0;
                 ctg++;
+                if constexpr (STS) ctg_start = next_start;
                 next_start = (ctg + 1 < d.n_contigs) ? (uint32_t)d.contig_off[ctg + 1] : 0xFFFFFFFFu;
             }
             const uint32_t orig = (dr >> (i * 8)) & 255u;
             const uint32_t cov = cover[i];
+            if constexpr (STS) if (p == ctg_start) sts4 |= 0x80u << (8 * i);
             if (cov == 0) {                                    // depth 0: always the original base
                 n_zero++;
                 po[i].packed = (orig == '-' ? 0u : 1u) | (orig << 16);
                 tlen += po[i].packed & 0xFFFFu;
+                if constexpr (STS) sts4 |= (prm.min_depth > 0 ? 0u : 2u) << (8 * i);
                 if (vp.dbg) {                                  // min_depth > 0: low_depth; min_depth == 0: A,C,G,T all "valid" -> multiple
                     pp_debug_pos r;
                     memset(&r, 0, sizeof r);
@@ -1757,14 +1771,15 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             tdepth += depth;
             uint32_t cA = sh.ex[0][rel], cC = sh.ex[1][rel], cG = sh.ex[2][rel], cT = sh.ex[3][rel];
             const uint32_t cDel = sh.del[rel], n_other = sh.oth[rel];
-            if ((cA | cC | cG | cT | cDel | n_other) == 0 && !vp.dbg) {
+            // (status mode: every covered position votes, its status being what the shortcuts below do not decide)
+            if ((cA | cC | cG | cT | cDel | n_other) == 0 && !vp.dbg && !STS) {
                 // every covering entry equals the draft base: the only allele with a non-zero count is the draft's own, so
                 // whatever the thresholds say (kept, too_close, low_depth, ...) the emitted base is the original
                 po[i].packed = (orig == '-' ? 0u : 1u) | (orig << 16);
                 tlen += po[i].packed & 0xFFFFu;
                 continue;
             }
-            if (!vp.dbg) {
+            if (!vp.dbg && !STS) {
                 // The emitted base differs from the draft only if an allele OTHER than the draft's reaches the valid threshold
                 // max(min_depth, round(depth * fraction_valid)) (pileup.rs:70-72,114-129).  No such allele can when the largest
                 // non-draft count is below min_depth, or below depth * fraction_valid by more than rounding can bridge: the
@@ -1784,7 +1799,9 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             po[i] = vote_position<BITS, CHG>(oc, prm, p, orig, vdepth, cA, cC, cG, cT, cDel, matched, n_other, vp);
             n_changed += (po[i].packed >> 24) & 1u;
             tlen += po[i].packed & 0xFFFFu;
+            if constexpr (STS) sts4 |= ((po[i].packed >> 26) & 7u) << (8 * i);
         }
+        if constexpr (STS) *reinterpret_cast<uint32_t*>(vp.sts + p0) = sts4;
         {   // per-contig statistics: one atomic per warp when the whole warp sits in one contig (nearly always)
             const uint32_t ctg0 = __shfl_sync(0xffffffffu, ctg, 0);
             if (__ballot_sync(0xffffffffu, ctg != ctg0) == 0u) {
@@ -1839,10 +1856,75 @@ static_assert(TL_PER_THREAD == 4, "the verdict store packs four positions per th
 #if !defined(PP_EMULATE)
 // One CTA per SM: built for sm_90a, the body needs ~100 registers per thread.  Capped at 64 for two CTAs per SM it spills, and on an
 // H100 (400 W) the tile kernel took 0.79 ms per 5 Mbp x 100x call that way against 0.71 ms with one CTA per SM.
-template <int BITS, bool CHG>
+template <int BITS, bool CHG, bool STS>
 __global__ void __launch_bounds__(TL_THREADS, 1) k_tile(DevData d, VoteParams vp) {
     extern __shared__ __align__(16) unsigned char tile_smem[];
-    tile_body<BITS, CHG>(d, vp, *reinterpret_cast<TileShared*>(tile_smem));
+    tile_body<BITS, CHG, STS>(d, vp, *reinterpret_cast<TileShared*>(tile_smem));
+}
+#endif
+
+// ------------------------------------------------------------------------------------------------------
+// k_status_heads / k_status_runs: k_tile's status bytes (VoteParams::sts) -> runs of equal status.  Position p starts a run where a
+// contig starts or where its status differs from position p - 1's.  CTA b looks at positions [b, b + 1) * SR_CHUNK: the first kernel
+// counts its runs, an exclusive scan of the counts gives each CTA its first run (and the total, so that the run arrays are sized
+// exactly), the second writes (start, status) of its runs in position order.  The status array is padded to whole SR_CHUNKs.
+// ------------------------------------------------------------------------------------------------------
+#define SR_THREADS 256
+#define SR_PER_THREAD 16
+#define SR_CHUNK (SR_THREADS * SR_PER_THREAD)
+static_assert(SR_CHUNK % TL_T == 0, "the status array padded to whole SR_CHUNKs also holds k_tile's whole tiles");
+struct RunShared {
+    unsigned long long s_warp[SR_THREADS / 32];
+    unsigned long long s_total;
+};
+
+// bit i: position p0 + i (< G) starts a run; *w receives the sixteen status bytes
+__device__ __forceinline__ uint32_t status_heads(const uint8_t* sts, uint32_t G, uint32_t p0, uint32_t w[4]) {
+    if (p0 >= G) return 0;
+    const uint4 q = *reinterpret_cast<const uint4*>(sts + p0);
+    w[0] = q.x; w[1] = q.y; w[2] = q.z; w[3] = q.w;
+    uint32_t prev = p0 ? sts[p0 - 1] : 0u;                   // (position 0 starts contig 0: its byte has bit 7)
+    uint32_t m = 0;
+#pragma unroll
+    for (int i = 0; i < SR_PER_THREAD; ++i) {
+        const uint32_t s = (w[i >> 2] >> (8 * (i & 3))) & 255u;
+        if (p0 + i < G && ((s & 0x80u) || ((s ^ prev) & 7u))) m |= 1u << i;
+        prev = s;
+    }
+    return m;
+}
+
+__device__ __forceinline__ void status_heads_body(const uint8_t* sts, uint32_t G, uint32_t* count, RunShared& sh) {
+    uint32_t w[4];
+    const uint32_t m = status_heads(sts, G, blockIdx.x * SR_CHUNK + threadIdx.x * SR_PER_THREAD, w);
+    block_exscan<SR_THREADS>((unsigned long long)__popc(m), sh.s_warp, &sh.s_total);
+    if (threadIdx.x == 0) count[blockIdx.x] = (uint32_t)sh.s_total;
+}
+
+// first[b]: the exclusive scan of the counts
+__device__ __forceinline__ void status_runs_body(const uint8_t* sts, uint32_t G, const uint32_t* first, uint32_t* start, uint8_t* status,
+                                                 RunShared& sh) {
+    uint32_t w[4];
+    const uint32_t p0 = blockIdx.x * SR_CHUNK + threadIdx.x * SR_PER_THREAD;
+    uint32_t m = status_heads(sts, G, p0, w);
+    uint32_t o = first[blockIdx.x] + (uint32_t)block_exscan<SR_THREADS>((unsigned long long)__popc(m), sh.s_warp, &sh.s_total);
+    while (m) {
+        const int i = __ffs(m) - 1;
+        m &= m - 1;
+        start[o] = p0 + i;
+        status[o] = (uint8_t)((w[i >> 2] >> (8 * (i & 3))) & 7u);
+        o++;
+    }
+}
+
+#if !defined(PP_EMULATE)
+__global__ void __launch_bounds__(SR_THREADS) k_status_heads(const uint8_t* sts, uint32_t G, uint32_t* count) {
+    __shared__ RunShared sh;
+    status_heads_body(sts, G, count, sh);
+}
+__global__ void __launch_bounds__(SR_THREADS) k_status_runs(const uint8_t* sts, uint32_t G, const uint32_t* first, uint32_t* start, uint8_t* status) {
+    __shared__ RunShared sh;
+    status_runs_body(sts, G, first, start, status, sh);
 }
 #endif
 

@@ -376,22 +376,55 @@ static const char* err_text(unsigned code) {
     }
 }
 
+// --status-bed: k_tile's status bytes, padded to whole CTAs of k_status_heads / k_status_runs (which load 16 bytes per thread)
+static size_t status_bytes(uint64_t G) { return (size_t)((G + SR_CHUNK - 1) / SR_CHUNK) * SR_CHUNK + 16; }
+
+// The status bytes of a call -> its runs in B_RUNSTART / B_RUNSTS, sized from the count (ctx->n_runs).
+static int status_runs(pp_ctx* ctx, const uint8_t* sts) {
+    cudaStream_t s = ctx->stream;
+    const uint32_t G = (uint32_t)ctx->G, n_blk = (uint32_t)((ctx->G + SR_CHUNK - 1) / SR_CHUNK);
+    CK(ctx->b[B_RUNFIRST].ensure(((size_t)n_blk + 1) * 4));
+    uint32_t* first = ctx->b[B_RUNFIRST].as<uint32_t>();
+    CK(cudaMemsetAsync(first + n_blk, 0, 4, s));
+    if (n_blk) k_status_heads<<<n_blk, SR_THREADS, 0, s>>>(sts, G, first);
+    size_t tb = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, first, first, (int)n_blk + 1, s));
+    CK(ctx->b[B_CUBTMP].ensure(tb + 256));
+    tb = ctx->b[B_CUBTMP].cap;
+    CK(cub::DeviceScan::ExclusiveSum(ctx->b[B_CUBTMP].p, tb, first, first, (int)n_blk + 1, s));
+    uint32_t n = 0;
+    CK(cudaMemcpyAsync(&n, first + n_blk, 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    CK(ctx->b[B_RUNSTART].ensure((size_t)n * 4 + 4)); CK(ctx->b[B_RUNSTS].ensure((size_t)n + 4));
+    if (n_blk) k_status_runs<<<n_blk, SR_THREADS, 0, s>>>(sts, G, first, ctx->b[B_RUNSTART].as<uint32_t>(), ctx->b[B_RUNSTS].as<uint8_t>());
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+    ctx->n_runs = n;
+    ctx->have_status = true;
+    return PP_OK;
+}
+
 template <int BITS>
 static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result* res) {
     cudaStream_t s = ctx->stream;
     const uint64_t G = ctx->G, n_aln = ctx->n_aln;
     const uint32_t n_tiles = (uint32_t)((G + TL_T - 1) / TL_T);              // = vote / compaction chunks
     const size_t padG = (size_t)n_tiles * TL_T + 16;                          // k_tile / k_compact move whole chunks with vector accesses
-    ctx->have_changes = false;
+    ctx->have_changes = ctx->have_status = false;
 
     CK(ctx->b[B_OUTOFF].ensure(((size_t)ctx->n_contigs + 1) * 8));
     CK(ctx->b[B_RES].ensure(padG * 2)); CK(ctx->b[B_RECAT].ensure((G + 1) * 4)); CK(ctx->b[B_CHUNKDELTA].ensure((size_t)n_tiles * 8));
     CK(ctx->b[B_PARAMS].ensure(sizeof(DevParams)));
     if (!ctx->tile_attr_set) {
-        CK(cudaFuncSetAttribute(k_tile<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<4, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<8, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<8, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<4, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<8, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        CK(cudaFuncSetAttribute(k_tile<8, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
         ctx->tile_attr_set = true;
     }
 
@@ -467,12 +500,15 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
             CK(ctx->b[B_CHG].ensure((size_t)ctx->chg_cap * sizeof(pp_debug_pos))); CK(ctx->b[B_CHGPOS].ensure((size_t)ctx->chg_cap * 4));
             vp.chg = ctx->b[B_CHG].as<pp_debug_pos>(); vp.chg_pos = ctx->b[B_CHGPOS].as<uint32_t>(); vp.chg_cap = ctx->chg_cap;
         }
+        vp.sts = nullptr;
+        if (ctx->status_on) { CK(ctx->b[B_STS].ensure(status_bytes(G))); vp.sts = ctx->b[B_STS].as<uint8_t>(); }
         {
+            auto kt = vp.chg ? (vp.sts ? k_tile<BITS, true, true> : k_tile<BITS, true, false>)
+                             : (vp.sts ? k_tile<BITS, false, true> : k_tile<BITS, false, false>);
             int occ = 1;
-            CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, vp.chg ? k_tile<BITS, true> : k_tile<BITS, false>, TL_THREADS, sizeof(TileShared)));
+            CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kt, TL_THREADS, sizeof(TileShared)));
             const uint32_t grid = std::min<uint32_t>(n_tiles, (uint32_t)ctx->sm_count * (uint32_t)std::max(occ, 1));   // persistent: tiles by ticket
-            if (vp.chg) k_tile<BITS, true><<<grid, TL_THREADS, sizeof(TileShared), s>>>(d, vp);
-            else k_tile<BITS, false><<<grid, TL_THREADS, sizeof(TileShared), s>>>(d, vp);
+            kt<<<grid, TL_THREADS, sizeof(TileShared), s>>>(d, vp);
             ctx->launches++;
         }
         // ---- stage 4: compaction
@@ -513,6 +549,10 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
 
         ctx->have_debug = ctx->debug_on; ctx->last_head = d.oth_head; ctx->last_nodes = std::min(hs.node_count, node_cap);
         ctx->have_changes = ctx->changes_on; ctx->n_changes = ctx->changes_on ? hs.n_changes : 0; ctx->chg_pool = -1;
+        if (ctx->status_on) {
+            const int rc = status_runs(ctx, vp.sts);
+            if (rc != PP_OK) return rc;
+        }
         res->out_len = hs.out_len;
         res->n_aln_used = hs.n_used;
         res->error_aln = -1;
@@ -705,5 +745,39 @@ extern "C" int pp_polish_changes_fetch(pp_ctx* ctx, uint64_t row_cap, uint64_t* 
     for (uint32_t i = 0; i < n; ++i) order[i] = i;
     std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return p[a] < p[b]; });
     for (uint32_t i = 0; i < n; ++i) { pos[i] = p[order[i]]; rows[i] = r[order[i]]; pool_off[i] = o[order[i]]; }
+    return PP_OK;
+}
+
+extern "C" int pp_polish_set_status(pp_ctx* ctx, int on) {
+    if (!ctx) return PP_ERR_ARG;
+    ctx->status_on = on == 1;           // 2 = stop recording but keep the last call's runs readable
+    if (on != 1) { CK(cudaSetDevice(ctx->device)); ctx->b[B_STS].release(); ctx->b[B_RUNFIRST].release(); }
+    if (on == 0) { ctx->have_status = false; ctx->b[B_RUNSTART].release(); ctx->b[B_RUNSTS].release(); }
+    return PP_OK;
+}
+
+extern "C" int pp_set_status_file(pp_ctx* ctx, const char* path) {
+    if (!ctx) return PP_ERR_ARG;
+    ctx->status_path = path ? path : "";
+    return PP_OK;
+}
+const char* pp_ctx_status_file(pp_ctx* ctx) { return ctx->status_path.c_str(); }
+
+extern "C" int pp_polish_status_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint8_t* status, uint64_t* n_runs) {
+    if (!ctx) return PP_ERR_ARG;
+    if (!ctx->have_status) return ctx->fail(PP_ERR_ARG, "pp_polish_status_fetch: the last polish did not record status (pp_polish_set_status)");
+    if (!n_runs) return ctx->fail(PP_ERR_ARG, "pp_polish_status_fetch: null size pointer");
+    const uint32_t n = ctx->n_runs;
+    *n_runs = n;
+    if (run_cap == 0 && n > 0) return PP_OK;                                                   // size query
+    if (run_cap < n || (n && (!start || !status))) return ctx->fail(PP_ERR_ARG, "pp_polish_status_fetch: buffers too small");
+    CK(cudaSetDevice(ctx->device));
+    std::vector<uint32_t> st(n);
+    if (n) {
+        CK(cudaMemcpyAsync(st.data(), ctx->b[B_RUNSTART].p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(status, ctx->b[B_RUNSTS].p, n, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::copy(st.begin(), st.end(), start);
     return PP_OK;
 }

@@ -31,7 +31,7 @@ struct DevBuf {
 enum { B_CONTIG, B_REFSTART, B_READID, B_SEQOFF, B_SEQLEN, B_CIGOFF, B_NCIG, B_NM, B_FLAGS, B_CIGOPS, B_SEQPOOL,
        B_DRAFT, B_CTGOFF, B_ZEROPOOL, B_RECS, B_KEY, B_VAL, B_SKEY, B_SVAL, B_BINSTART, B_SREC, B_SSEQ, B_KF, B_NK, B_TILEORDER, B_ERRC, B_GQ, B_HEADS, B_NODES, B_CUBTMP, B_SEQ2, B_OUT,
        B_OUTOFF, B_DEBUG, B_RES, B_RECAT, B_CHUNKDELTA, B_PARAMS, B_SCRATCH, B_SCRATCH2,
-       B_CHG, B_CHGPOS, B_STRPOS, B_STRPOOL, B_STROFF,
+       B_CHG, B_CHGPOS, B_STRPOS, B_STRPOOL, B_STROFF, B_STS, B_RUNFIRST, B_RUNSTART, B_RUNSTS,
        B_TOKLINE, B_TOKTMP, B_TOKNAMES, B_COUNT };
 
 struct pp_ctx {
@@ -65,6 +65,10 @@ struct pp_ctx {
     uint32_t chg_cap = 0, n_changes = 0;
     int64_t chg_pool = -1;                // bytes of the change rows' allele strings in B_STRPOOL, -1 = not made yet
     std::string changes_path;             // pp_set_changes_file: the report the file-level commands also write
+    // --status-bed (pp_polish_set_status): the status runs of the last call (B_RUNSTART / B_RUNSTS, exactly n_runs long)
+    bool status_on = false, have_status = false;
+    uint32_t n_runs = 0;
+    std::string status_path;              // pp_set_status_file: the BED the file-level commands also write
     TokState* tok = nullptr;              // SAM tokeniser state (tok_kernels.cu), created on first use
     int parser = 0;                       // pp_set_parser: 0 device tokeniser where possible, 1 host packer only
 
