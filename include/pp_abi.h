@@ -226,6 +226,12 @@ int pp_polish_status_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint8
  * copied. */
 int pp_set_status_file(pp_ctx* ctx, const char* path);
 
+/* The VCF (--vcf): the same whole-command calls made with `ctx` (ctxs[0]) as their context also write the polish's edits to the draft
+ * to `path` as VCF 4.2 records, plain text with no sample columns, that rebuild the polished FASTA byte for byte when applied to the
+ * draft.  Built on the host from the change report's rows (pp_polish_changes_fetch) and the draft; the records' rules are in
+ * polypolish_b200/csrc/vcf_records.h.  NULL or "" switches it off (the default).  The path is copied. */
+int pp_set_vcf_file(pp_ctx* ctx, const char* path);
+
 /* ------------------------------------------------------------------------------------------------------
  * filter (filter.rs).  One record per ALIGNED line of one mate's SAM file, in file order.
  * Replaces get_insert_size_thresholds (filter.rs:148-186) and alignment_pass_qc (filter.rs:352-377).

@@ -160,6 +160,7 @@ def lib():
                                           C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.pp_polish_set_status.argtypes = [C.c_void_p, C.c_int]
     L.pp_set_status_file.argtypes = [C.c_void_p, C.c_char_p]
+    L.pp_set_vcf_file.argtypes = [C.c_void_p, C.c_char_p]
     L.pp_polish_status_fetch.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     if hasattr(L, "pp_filter"):
         L.pp_filter.argtypes = [C.c_void_p, C.POINTER(FilterMate), C.POINTER(FilterMate), C.POINTER(FilterParams),
@@ -545,19 +546,25 @@ class Context:
         """pp_set_status_file: the file-level calls on this context also write the status runs as BED to `path` (None: off)."""
         lib().pp_set_status_file(self.h, str(path).encode() if path else None)
 
-    def polish_files(self, assembly, sams, debug=None, changes=None, status=None, verbose=False, **opts):
+    def set_vcf_file(self, path):
+        """pp_set_vcf_file: the file-level calls on this context also write the polish's edits to the draft as VCF to `path` (None: off)."""
+        lib().pp_set_vcf_file(self.h, str(path).encode() if path else None)
+
+    def polish_files(self, assembly, sams, debug=None, changes=None, status=None, vcf=None, verbose=False, **opts):
         prm = _params(**opts)
         arr = (C.c_char_p * max(1, len(sams)))(*[str(s).encode() for s in sams])
         out = C.c_void_p()
         n = C.c_uint64()
         self.set_changes_file(changes)
         self.set_status_file(status)
+        self.set_vcf_file(vcf)
         try:
             rc = lib().pp_polish_files(self.h, str(assembly).encode(), arr, len(sams), C.byref(prm),
                                        str(debug).encode() if debug else None, C.byref(out), C.byref(n), int(verbose))
         finally:
             self.set_changes_file(None)
             self.set_status_file(None)
+            self.set_vcf_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
@@ -565,7 +572,7 @@ class Context:
         return data
 
     def filter_polish_files(self, assembly, in1, in2, out1=None, out2=None, orientation="auto", low=0.1, high=99.9, verbose=False, changes=None,
-                            status=None, **opts):
+                            status=None, vcf=None, **opts):
         """pp_filter_polish_files: `filter` then `polish` in one call (the filtered SAM files are written only when named)."""
         L = lib()
         L.pp_filter_polish_files.argtypes = [C.c_void_p] + [C.c_char_p] * 6 + [C.c_double, C.c_double, C.POINTER(PolishParams),
@@ -574,6 +581,7 @@ class Context:
         out, n = C.c_void_p(), C.c_uint64()
         self.set_changes_file(changes)
         self.set_status_file(status)
+        self.set_vcf_file(vcf)
         try:
             rc = L.pp_filter_polish_files(self.h, str(assembly).encode(), str(in1).encode(), str(in2).encode(),
                                           str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
@@ -581,6 +589,7 @@ class Context:
         finally:
             self.set_changes_file(None)
             self.set_status_file(None)
+            self.set_vcf_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
@@ -619,11 +628,11 @@ def polish_files(assembly, sams, device=0, **kw):
 
 
 def polish(assembly, sam, debug=None, fraction_invalid=0.2, fraction_valid=0.5, max_errors=10, min_depth=5,
-           careful=False, device=0, changes=None, status=None):
+           careful=False, device=0, changes=None, status=None, vcf=None):
     """`polypolish polish` (main.rs:78-108, polish.rs:26-38): returns the bytes the reference prints to stdout.  changes: also
     write the change report (the --debug rows of the changed positions) to this file; status: also write every position's status
-    as BED runs (--status-bed) to this file."""
-    return polish_files(assembly, list(sam), device=device, debug=debug, changes=changes, status=status, fraction_invalid=fraction_invalid,
+    as BED runs (--status-bed) to this file; vcf: also write the edits to the draft as VCF (--vcf) to this file."""
+    return polish_files(assembly, list(sam), device=device, debug=debug, changes=changes, status=status, vcf=vcf, fraction_invalid=fraction_invalid,
                         fraction_valid=fraction_valid, max_errors=max_errors, min_depth=min_depth, careful=careful)
 
 
@@ -821,11 +830,11 @@ class TwoBit:
             pass
 
 
-def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, contexts=None, changes=None, status=None, **opts):
+def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, contexts=None, changes=None, status=None, vcf=None, **opts):
     """pp_polish_files_multi: contigs shard over one context per entry of `devices` (entries may repeat), or over the given `contexts`
     (reused across calls like a long-running host would).  parser 0 (default): every context tokenises the text itself and keeps its
     shard (pp_tok_set_shard); 1: host packer + host sharder.  changes: also write the change report to this file (every context
-    reports its own contigs); status: also write the status runs as BED to this file."""
+    reports its own contigs); status: also write the status runs as BED to this file; vcf: also write the edits as VCF to this file."""
     L = lib()
     L.pp_polish_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_char_p, C.POINTER(C.c_char_p), C.c_int,
                                         C.POINTER(PolishParams), C.c_char_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
@@ -838,12 +847,14 @@ def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, co
         out, n = C.c_void_p(), C.c_uint64()
         ctxs[0].set_changes_file(changes)
         ctxs[0].set_status_file(status)
+        ctxs[0].set_vcf_file(vcf)
         try:
             rc = L.pp_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), arr, len(sams), C.byref(prm), None,
                                          C.byref(out), C.byref(n), int(verbose))
         finally:
             ctxs[0].set_changes_file(None)
             ctxs[0].set_status_file(None)
+            ctxs[0].set_vcf_file(None)
         if rc != PP_OK:
             raise ctxs[0]._err(rc)
         data = C.string_at(out, n.value)
@@ -881,10 +892,10 @@ def filter_files_multi(in1, in2, out1, out2, orientation="auto", low=0.1, high=9
 
 
 def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientation="auto", low=0.1, high=99.9, devices=None, verbose=False,
-                              parser=0, contexts=None, changes=None, status=None, **opts):
+                              parser=0, contexts=None, changes=None, status=None, vcf=None, **opts):
     """pp_filter_polish_files_multi: `filter` then `polish` in one call over one context per entry of `devices` (entries may repeat) or
     over the given `contexts`; the filtered SAM files are written only when named.  changes: also write the change report to this file;
-    status: also write the status runs as BED to this file."""
+    status: also write the status runs as BED to this file; vcf: also write the edits as VCF to this file."""
     L = lib()
     L.pp_filter_polish_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int] + [C.c_char_p] * 6 + [
         C.c_double, C.c_double, C.POINTER(PolishParams), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
@@ -894,6 +905,7 @@ def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientat
         out, n = C.c_void_p(), C.c_uint64()
         ctxs[0].set_changes_file(changes)
         ctxs[0].set_status_file(status)
+        ctxs[0].set_vcf_file(vcf)
         try:
             rc = L.pp_filter_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), str(in1).encode(), str(in2).encode(),
                                                 str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
@@ -901,6 +913,7 @@ def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientat
         finally:
             ctxs[0].set_changes_file(None)
             ctxs[0].set_status_file(None)
+            ctxs[0].set_vcf_file(None)
         if rc != PP_OK:
             raise ctxs[0]._err(rc)
         data = C.string_at(out, n.value)

@@ -26,7 +26,7 @@ def _stale(target, sources):
     if not os.path.exists(target):
         return True
     t = os.path.getmtime(target)
-    deps = list(sources) + [os.path.join(CSRC, "pp_internal.h"), os.path.join(CSRC, "nib_utils.h"), os.path.join(CSRC, "pp_ctx.cuh"), os.path.join(CSRC, "polish_dev.cuh"), os.path.join(CSRC, "debug_rows.h"),
+    deps = list(sources) + [os.path.join(CSRC, "pp_internal.h"), os.path.join(CSRC, "nib_utils.h"), os.path.join(CSRC, "pp_ctx.cuh"), os.path.join(CSRC, "polish_dev.cuh"), os.path.join(CSRC, "debug_rows.h"), os.path.join(CSRC, "vcf_records.h"),
                             os.path.join(CSRC, "tok_line.h"), os.path.join(CSRC, "tok_table.h"), os.path.join(CSRC, "filter_dev.h"), os.path.join(CSRC, "tok_strip.h"), os.path.join(ROOT, "include", "pp_abi.h"),
                             os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))

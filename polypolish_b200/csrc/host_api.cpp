@@ -15,12 +15,15 @@
 #include <algorithm>
 #include <memory>
 #include <string>
+#include <string_view>
 #include <thread>
 #include <utility>
 #include <vector>
 
 #include "debug_rows.h"
+#include "pp_ctx.cuh"
 #include "pp_internal.h"
+#include "vcf_records.h"
 
 namespace {
 
@@ -546,17 +549,24 @@ static std::pair<uint32_t, uint64_t> input_position(const ShardJob& j, bool one_
     return {one_job ? lc : j.contig_map[lc], pos - j.contigs.off[lc]};
 }
 
-// --changes: the --debug rows of the changed positions, in the input FASTA's contig order, then position order.  Every job reports
-// the rows of its own contigs (pp_polish_changes_fetch); they are merged here.  PP_ERR_IO: the file could not be written; another
-// error: its message is on ctx.
-static int write_changes(pp_ctx* ctx, const pp_fasta* fa, const std::vector<ShardJob>& jobs, FILE* f) {
+// --changes / --vcf: the change rows of every job, merged in the input FASTA's contig order, then position order.  Every job reports
+// the rows of its own contigs (pp_polish_changes_fetch).
+struct ChangeRows {
     struct Fetched { std::vector<uint64_t> pos, off; std::vector<pp_debug_pos> rows; std::vector<uint8_t> pool; };
     struct Row { uint32_t contig; uint64_t pos; uint32_t job; uint64_t i; };
-    std::vector<Fetched> got(jobs.size());
+    std::vector<Fetched> got;
     std::vector<Row> order;
+    const pp_debug_pos& rec(const Row& r) const { return got[r.job].rows[r.i]; }
+    const uint8_t* alleles(const Row& r) const { return got[r.job].pool.data() + got[r.job].off[r.i]; }
+};
+
+// PP_OK, or an error whose message is on ctx.
+static int fetch_changes(pp_ctx* ctx, const std::vector<ShardJob>& jobs, ChangeRows& cr) {
+    cr.got.assign(jobs.size(), {});
+    cr.order.clear();
     for (uint32_t s = 0; s < jobs.size(); ++s) {
         const ShardJob& j = jobs[s];
-        Fetched& g = got[s];
+        ChangeRows::Fetched& g = cr.got[s];
         uint64_t n = 0, bytes = 0;
         int rc = pp_polish_changes_fetch(j.ctx, 0, nullptr, nullptr, nullptr, nullptr, 0, &n, &bytes);
         if (rc == PP_OK) {
@@ -566,15 +576,60 @@ static int write_changes(pp_ctx* ctx, const pp_fasta* fa, const std::vector<Shar
         if (rc != PP_OK) return pp_ctx_fail(ctx, rc, std::string(pp_last_error(j.ctx)).c_str());
         for (uint64_t i = 0; i < n; ++i) {
             const auto cp = input_position(j, jobs.size() == 1, g.pos[i]);
-            order.push_back({cp.first, cp.second, s, i});
+            cr.order.push_back({cp.first, cp.second, s, i});
         }
     }
-    std::sort(order.begin(), order.end(), [](const Row& a, const Row& b) { return a.contig != b.contig ? a.contig < b.contig : a.pos < b.pos; });
+    std::sort(cr.order.begin(), cr.order.end(), [](const ChangeRows::Row& a, const ChangeRows::Row& b) {
+        return a.contig != b.contig ? a.contig < b.contig : a.pos < b.pos;
+    });
+    return PP_OK;
+}
+
+// --changes: the --debug header, then the --debug rows of the changed positions.  PP_ERR_IO: the file could not be written.
+static int write_changes(const pp_fasta* fa, const ChangeRows& cr, FILE* f) {
     std::string buf = pp::DEBUG_HEADER;
     pp::DebugRows rows;
-    for (const Row& r : order) {
-        const Fetched& g = got[r.job];
-        rows.add(buf, pp_fasta_name(fa, r.contig), r.pos, g.rows[r.i], g.pool.data() + g.off[r.i]);
+    for (const ChangeRows::Row& r : cr.order) rows.add(buf, pp_fasta_name(fa, r.contig), r.pos, cr.rec(r), cr.alleles(r));
+    return fwrite(buf.data(), 1, buf.size(), f) == buf.size() ? PP_OK : PP_ERR_IO;
+}
+
+// The allele a change row emits and its count in the row's --debug pileup column: count[0..3] for A/C/G/T, count[4] for "-", else
+// the matching entry of the row's allele strings (`al`, in k_allele_strings' format; a changed row never emits the draft's own base,
+// count[5]).  false: the allele is not in the pileup.
+static bool emitted_allele(const pp_debug_pos& r, const uint8_t* al, std::string_view& allele, uint32_t& support) {
+    const uint32_t n = pp::get_u32(al);
+    const uint8_t* q = al + 4;
+    for (uint32_t i = 0; i < n; ++i) q += 8 + pp::get_u32(q + 4);
+    allele = r.new_node != 0xFFFFFFFFu ? std::string_view((const char*)q + 4, pp::get_u32(q)) : std::string_view((const char*)&r.new_char, 1);
+    static const char* const single = "ACGT-";
+    if (allele.size() == 1 && allele[0])
+        if (const char* b = strchr(single, allele[0])) { support = r.count[b - single]; return true; }
+    q = al + 4;
+    for (uint32_t i = 0; i < n; ++i, q += 8 + pp::get_u32(q + 4))
+        if (std::string_view((const char*)q + 8, pp::get_u32(q + 4)) == allele) { support = pp::get_u32(q); return true; }
+    return false;
+}
+
+// --vcf: the header, then per contig in the input FASTA's order the records vcf_records.h makes of its draft and its change rows.
+// PP_ERR_IO: the file could not be written; another error: its message is on ctx.
+static int write_vcf(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const ChangeRows& cr, FILE* f) {
+    std::string buf;
+    pp::vcf_header_begin(buf);
+    for (uint32_t c = 0; c < contigs.n_contigs; ++c) pp::vcf_header_contig(buf, pp_fasta_name(fa, c), contigs.off[c + 1] - contigs.off[c]);
+    pp::vcf_header_end(buf);
+    std::vector<pp::VcfChange> ch;
+    size_t k = 0;
+    for (uint32_t c = 0; c < contigs.n_contigs; ++c) {
+        ch.clear();
+        for (; k < cr.order.size() && cr.order[k].contig == c; ++k) {
+            const ChangeRows::Row& r = cr.order[k];
+            pp::VcfChange v{r.pos, {}, cr.rec(r).depth, 0};
+            if (!emitted_allele(cr.rec(r), cr.alleles(r), v.allele, v.support))
+                return pp_ctx_fail(ctx, PP_ERR_CUDA, ("--vcf: the allele emitted at " + std::string(pp_fasta_name(fa, c)) + ":" +
+                                                      std::to_string(r.pos) + " is not in its pileup").c_str());
+            ch.push_back(v);
+        }
+        pp::vcf_records(buf, pp_fasta_name(fa, c), contigs.bases + contigs.off[c], contigs.off[c + 1] - contigs.off[c], ch.data(), ch.size());
     }
     return fwrite(buf.data(), 1, buf.size(), f) == buf.size() ? PP_OK : PP_ERR_IO;
 }
@@ -641,32 +696,23 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     for (int i = 0; i < n_sams; ++i)
         if (!pp::file_exists(sams[i])) return pp_ctx_fail(ctx, PP_ERR_INPUT, ("\"" + std::string(sams[i]) + "\" file does not exist").c_str());
     const bool debug = debug_path && debug_path[0];
-    FILE* debug_file = nullptr;
-    if (debug) {                                          // create_debug_file polish.rs:230-244
-        debug_file = fopen(debug_path, "wb");
-        if (!debug_file) return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + std::string(debug_path) + "\"").c_str());
-    }
-    const std::string changes_path = pp_ctx_changes_file(ctx);
-    const bool changes = !changes_path.empty();
-    FILE* changes_file = nullptr;
-    if (changes) {                                        // worded like --debug's
-        changes_file = fopen(changes_path.c_str(), "wb");
-        if (!changes_file) { if (debug_file) fclose(debug_file); return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + changes_path + "\"").c_str()); }
-    }
-    const std::string status_path = pp_ctx_status_file(ctx);
-    const bool status = !status_path.empty();
-    FILE* status_file = nullptr;
-    if (status) {
-        status_file = fopen(status_path.c_str(), "wb");
-        if (!status_file) {
-            if (debug_file) fclose(debug_file);
-            if (changes_file) fclose(changes_file);
-            return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + status_path + "\"").c_str());
-        }
-    }
-    struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file}, closer2{changes_file}, closer3{status_file};
+    const std::string changes_path = pp_ctx_changes_file(ctx), status_path = pp_ctx_status_file(ctx), vcf_path = pp_ctx_vcf_file(ctx);
+    const bool changes = !changes_path.empty(), status = !status_path.empty(), vcf = !vcf_path.empty();
+    FILE *debug_file = nullptr, *changes_file = nullptr, *status_file = nullptr, *vcf_file = nullptr;
+    struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file}, closer2{changes_file}, closer3{status_file},
+        closer4{vcf_file};
+    // create_debug_file polish.rs:230-244; the other reports are worded like it
+    auto create = [ctx](const std::string& path, FILE*& file) {
+        file = fopen(path.c_str(), "wb");
+        return file ? PP_OK : pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + path + "\"").c_str());
+    };
+    int created = debug ? create(debug_path, debug_file) : PP_OK;
+    if (created == PP_OK && changes) created = create(changes_path, changes_file);
+    if (created == PP_OK && status) created = create(status_path, status_file);
+    if (created == PP_OK && vcf) created = create(vcf_path, vcf_file);
+    if (created != PP_OK) return created;
     Recording<pp_polish_set_debug> recording(&ctx, 1, debug);
-    Recording<pp_polish_set_changes> recording_changes(ctxs, n_ctx, changes);
+    Recording<pp_polish_set_changes> recording_changes(ctxs, n_ctx, changes || vcf);
     Recording<pp_polish_set_status> recording_status(ctxs, n_ctx, status);
 
     // the first SAM file starts streaming into HBM while the assembly is loaded
@@ -716,13 +762,19 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
         rc = write_debug_tsv(ctx, fa.get(), &contigs, debug_file);
         if (rc != PP_OK && rc != PP_ERR_CUDA) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + std::string(debug_path) + "\"").c_str());
     }
+    ChangeRows change_rows;
+    if (rc == PP_OK && (changes || vcf)) rc = fetch_changes(ctx, ld.jobs, change_rows);
     if (rc == PP_OK && changes) {
-        rc = write_changes(ctx, fa.get(), ld.jobs, changes_file);
+        rc = write_changes(fa.get(), change_rows, changes_file);
         if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + changes_path + "\"").c_str());
     }
     if (rc == PP_OK && status) {
         rc = write_status_bed(ctx, fa.get(), contigs, ld.jobs, status_file);
         if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + status_path + "\"").c_str());
+    }
+    if (rc == PP_OK && vcf) {
+        rc = write_vcf(ctx, fa.get(), contigs, change_rows, vcf_file);
+        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + vcf_path + "\"").c_str());
     }
     if (rc != PP_OK) return rc;
     recording.ok = recording_changes.ok = recording_status.ok = true;
@@ -794,6 +846,13 @@ extern "C" int pp_filter_polish_files_multi(pp_ctx* const* ctxs, int n_ctx, cons
     if (rc != PP_TOK_HOST) return rc;
     return pp_filter_polish_files(ctx, assembly, in1, in2, out1, out2, orientation, low, high, prm, out_fasta, out_len, verbose);
 }
+
+extern "C" int pp_set_vcf_file(pp_ctx* ctx, const char* path) {
+    if (!ctx) return PP_ERR_ARG;
+    ctx->vcf_path = path ? path : "";
+    return PP_OK;
+}
+const char* pp_ctx_vcf_file(pp_ctx* ctx) { return ctx->vcf_path.c_str(); }
 
 extern "C" int pp_polish_files(pp_ctx* ctx, const char* assembly, const char* const* sams, int n_sams,
                                const pp_polish_params* prm, const char* debug_path, char** out_fasta,

@@ -69,6 +69,7 @@ struct pp_ctx {
     bool status_on = false, have_status = false;
     uint32_t n_runs = 0;
     std::string status_path;              // pp_set_status_file: the BED the file-level commands also write
+    std::string vcf_path;                 // pp_set_vcf_file: the VCF the file-level commands also write (from the change rows)
     TokState* tok = nullptr;              // SAM tokeniser state (tok_kernels.cu), created on first use
     int parser = 0;                       // pp_set_parser: 0 device tokeniser where possible, 1 host packer only
 
