@@ -226,6 +226,20 @@ int pp_polish_status_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint8
  * copied. */
 int pp_set_status_file(pp_ctx* ctx, const char* path);
 
+/* The depth runs (--depth-bedgraph): every position's depth as the --debug depth column prints it ("%.1f" of the reference's sequential
+ * f64 sum of 1/k, pileup.rs:64, alignment.rs:297-303) as runs of equal printed depth.  Recording is off by default; like
+ * pp_polish_set_status it keeps the vote's shortcuts, and it costs eight bytes per position on the device while it is on.  Switch it on
+ * before the polish call (1 record, 2 stop but keep the last runs, 0 off). */
+int pp_polish_set_depth(pp_ctx* ctx, int on);
+/* runs of the last polish with recording on, in position order: start[i] = global position, tenths[i] = the printed depth times ten
+ * (12.3 -> 123); run i ends at start[i + 1] (or at total bp); every contig start begins a run.  Call once with run_cap = 0 for
+ * *n_runs. */
+int pp_polish_depth_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint64_t* tenths, uint64_t* n_runs);
+/* The whole-command calls (as pp_set_status_file) made with `ctx` (ctxs[0]) as their context also write the depth runs to `path` as
+ * bedGraph: "<contig>\t<start>\t<end>\t<depth>\n" per run, 0-based half-open, <depth> the --debug depth text, contigs in the assembly's
+ * order, no header or track line.  NULL or "" switches it off (the default).  The path is copied. */
+int pp_set_depth_file(pp_ctx* ctx, const char* path);
+
 /* The VCF (--vcf): the same whole-command calls made with `ctx` (ctxs[0]) as their context also write the polish's edits to the draft
  * to `path` as VCF 4.2 records, plain text with no sample columns, that rebuild the polished FASTA byte for byte when applied to the
  * draft.  Built on the host from the change report's rows (pp_polish_changes_fetch) and the draft; the records' rules are in

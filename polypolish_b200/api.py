@@ -162,6 +162,9 @@ def lib():
     L.pp_set_status_file.argtypes = [C.c_void_p, C.c_char_p]
     L.pp_set_vcf_file.argtypes = [C.c_void_p, C.c_char_p]
     L.pp_polish_status_fetch.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+    L.pp_polish_set_depth.argtypes = [C.c_void_p, C.c_int]
+    L.pp_set_depth_file.argtypes = [C.c_void_p, C.c_char_p]
+    L.pp_polish_depth_fetch.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
     if hasattr(L, "pp_filter"):
         L.pp_filter.argtypes = [C.c_void_p, C.POINTER(FilterMate), C.POINTER(FilterMate), C.POINTER(FilterParams),
                                 C.POINTER(FilterResult)]
@@ -378,9 +381,10 @@ class Context:
         self._nc = contigs.n_contigs
         self._G = int(np.ctypeslib.as_array(C.cast(contigs.off, C.POINTER(C.c_uint64)), shape=(contigs.n_contigs + 1,))[-1])
 
-    def polish_resident(self, fetch=True, changes=False, status=False, **opts):
+    def polish_resident(self, fetch=True, changes=False, status=False, depth_runs=False, **opts):
         """pp_polish_resident.  changes=True: the call also records the change report, returned under "changes" (changes_rows).
-        status=True: the call also records every position's status, returned as runs under "status" (status_runs)."""
+        status=True: the call also records every position's status, returned as runs under "status" (status_runs).
+        depth_runs=True: the call also records every position's printed depth, returned as runs under "depth" (depth_runs)."""
         prm = _params(**opts)
         cap = self._G + (1 << 20) if fetch else 0
         L = lib()
@@ -388,6 +392,8 @@ class Context:
             L.pp_polish_set_changes(self.h, 1)
         if status:
             L.pp_polish_set_status(self.h, 1)
+        if depth_runs:
+            L.pp_polish_set_depth(self.h, 1)
         ok = False
         try:
             for _ in range(2):
@@ -408,11 +414,15 @@ class Context:
                 L.pp_polish_set_changes(self.h, 2 if ok else 0)     # a failed call leaves nothing recording
             if status:
                 L.pp_polish_set_status(self.h, 2 if ok else 0)
+            if depth_runs:
+                L.pp_polish_set_depth(self.h, 2 if ok else 0)
         out = self._finish(res, keep, self._nc) if fetch else dict(n_aln_used=res.n_aln_used, out_len=res.out_len, timing=res.timing.as_dict())
         if changes:
             out["changes"] = self.changes_rows()
         if status:
             out["status"] = self.status_runs()
+        if depth_runs:
+            out["depth"] = self.depth_runs()
         return out
 
     def status_runs(self):
@@ -432,6 +442,23 @@ class Context:
         start, status = start[:n.value], status[:n.value]
         end = np.append(start[1:], np.uint64(self._G)).astype(np.uint64)
         return dict(start=start, end=end, status=status)
+
+    def depth_runs(self):
+        """The depth runs of the last polish with depth recorded (pp_polish_depth_fetch), in position order: numpy arrays "start" and
+        "end" (global positions, half-open) and "tenths" (the --debug depth text times ten: 12.3 -> 123)."""
+        L = lib()
+        n = C.c_uint64()
+        rc = L.pp_polish_depth_fetch(self.h, 0, None, None, C.byref(n))
+        if rc != PP_OK:
+            raise self._err(rc)
+        start, tenths = np.zeros(max(1, n.value), np.uint64), np.zeros(max(1, n.value), np.uint64)
+        if n.value:
+            rc = L.pp_polish_depth_fetch(self.h, n.value, start.ctypes.data, tenths.ctypes.data, C.byref(n))
+            if rc != PP_OK:
+                raise self._err(rc)
+        start, tenths = start[:n.value], tenths[:n.value]
+        end = np.append(start[1:], np.uint64(self._G)).astype(np.uint64)
+        return dict(start=start, end=end, tenths=tenths)
 
     def changes_rows(self):
         """The change report of the last polish with changes recorded (pp_polish_changes_fetch), in position order: one dict per
@@ -550,7 +577,11 @@ class Context:
         """pp_set_vcf_file: the file-level calls on this context also write the polish's edits to the draft as VCF to `path` (None: off)."""
         lib().pp_set_vcf_file(self.h, str(path).encode() if path else None)
 
-    def polish_files(self, assembly, sams, debug=None, changes=None, status=None, vcf=None, verbose=False, **opts):
+    def set_depth_file(self, path):
+        """pp_set_depth_file: the file-level calls on this context also write the depth runs as bedGraph to `path` (None: off)."""
+        lib().pp_set_depth_file(self.h, str(path).encode() if path else None)
+
+    def polish_files(self, assembly, sams, debug=None, changes=None, status=None, vcf=None, depth_bedgraph=None, verbose=False, **opts):
         prm = _params(**opts)
         arr = (C.c_char_p * max(1, len(sams)))(*[str(s).encode() for s in sams])
         out = C.c_void_p()
@@ -558,6 +589,7 @@ class Context:
         self.set_changes_file(changes)
         self.set_status_file(status)
         self.set_vcf_file(vcf)
+        self.set_depth_file(depth_bedgraph)
         try:
             rc = lib().pp_polish_files(self.h, str(assembly).encode(), arr, len(sams), C.byref(prm),
                                        str(debug).encode() if debug else None, C.byref(out), C.byref(n), int(verbose))
@@ -565,6 +597,7 @@ class Context:
             self.set_changes_file(None)
             self.set_status_file(None)
             self.set_vcf_file(None)
+            self.set_depth_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
@@ -572,7 +605,7 @@ class Context:
         return data
 
     def filter_polish_files(self, assembly, in1, in2, out1=None, out2=None, orientation="auto", low=0.1, high=99.9, verbose=False, changes=None,
-                            status=None, vcf=None, **opts):
+                            status=None, vcf=None, depth_bedgraph=None, **opts):
         """pp_filter_polish_files: `filter` then `polish` in one call (the filtered SAM files are written only when named)."""
         L = lib()
         L.pp_filter_polish_files.argtypes = [C.c_void_p] + [C.c_char_p] * 6 + [C.c_double, C.c_double, C.POINTER(PolishParams),
@@ -582,6 +615,7 @@ class Context:
         self.set_changes_file(changes)
         self.set_status_file(status)
         self.set_vcf_file(vcf)
+        self.set_depth_file(depth_bedgraph)
         try:
             rc = L.pp_filter_polish_files(self.h, str(assembly).encode(), str(in1).encode(), str(in2).encode(),
                                           str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
@@ -590,6 +624,7 @@ class Context:
             self.set_changes_file(None)
             self.set_status_file(None)
             self.set_vcf_file(None)
+            self.set_depth_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
@@ -628,11 +663,13 @@ def polish_files(assembly, sams, device=0, **kw):
 
 
 def polish(assembly, sam, debug=None, fraction_invalid=0.2, fraction_valid=0.5, max_errors=10, min_depth=5,
-           careful=False, device=0, changes=None, status=None, vcf=None):
+           careful=False, device=0, changes=None, status=None, vcf=None, depth_bedgraph=None):
     """`polypolish polish` (main.rs:78-108, polish.rs:26-38): returns the bytes the reference prints to stdout.  changes: also
     write the change report (the --debug rows of the changed positions) to this file; status: also write every position's status
-    as BED runs (--status-bed) to this file; vcf: also write the edits to the draft as VCF (--vcf) to this file."""
-    return polish_files(assembly, list(sam), device=device, debug=debug, changes=changes, status=status, vcf=vcf, fraction_invalid=fraction_invalid,
+    as BED runs (--status-bed) to this file; vcf: also write the edits to the draft as VCF (--vcf) to this file; depth_bedgraph: also
+    write every position's depth as bedGraph runs (--depth-bedgraph) to this file."""
+    return polish_files(assembly, list(sam), device=device, debug=debug, changes=changes, status=status, vcf=vcf,
+                        depth_bedgraph=depth_bedgraph, fraction_invalid=fraction_invalid,
                         fraction_valid=fraction_valid, max_errors=max_errors, min_depth=min_depth, careful=careful)
 
 
@@ -830,11 +867,13 @@ class TwoBit:
             pass
 
 
-def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, contexts=None, changes=None, status=None, vcf=None, **opts):
+def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, contexts=None, changes=None, status=None, vcf=None,
+                       depth_bedgraph=None, **opts):
     """pp_polish_files_multi: contigs shard over one context per entry of `devices` (entries may repeat), or over the given `contexts`
     (reused across calls like a long-running host would).  parser 0 (default): every context tokenises the text itself and keeps its
     shard (pp_tok_set_shard); 1: host packer + host sharder.  changes: also write the change report to this file (every context
-    reports its own contigs); status: also write the status runs as BED to this file; vcf: also write the edits as VCF to this file."""
+    reports its own contigs); status: also write the status runs as BED to this file; vcf: also write the edits as VCF to this file;
+    depth_bedgraph: also write the depth runs as bedGraph to this file."""
     L = lib()
     L.pp_polish_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_char_p, C.POINTER(C.c_char_p), C.c_int,
                                         C.POINTER(PolishParams), C.c_char_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
@@ -848,6 +887,7 @@ def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, co
         ctxs[0].set_changes_file(changes)
         ctxs[0].set_status_file(status)
         ctxs[0].set_vcf_file(vcf)
+        ctxs[0].set_depth_file(depth_bedgraph)
         try:
             rc = L.pp_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), arr, len(sams), C.byref(prm), None,
                                          C.byref(out), C.byref(n), int(verbose))
@@ -855,6 +895,7 @@ def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, co
             ctxs[0].set_changes_file(None)
             ctxs[0].set_status_file(None)
             ctxs[0].set_vcf_file(None)
+            ctxs[0].set_depth_file(None)
         if rc != PP_OK:
             raise ctxs[0]._err(rc)
         data = C.string_at(out, n.value)
@@ -892,10 +933,11 @@ def filter_files_multi(in1, in2, out1, out2, orientation="auto", low=0.1, high=9
 
 
 def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientation="auto", low=0.1, high=99.9, devices=None, verbose=False,
-                              parser=0, contexts=None, changes=None, status=None, vcf=None, **opts):
+                              parser=0, contexts=None, changes=None, status=None, vcf=None, depth_bedgraph=None, **opts):
     """pp_filter_polish_files_multi: `filter` then `polish` in one call over one context per entry of `devices` (entries may repeat) or
     over the given `contexts`; the filtered SAM files are written only when named.  changes: also write the change report to this file;
-    status: also write the status runs as BED to this file; vcf: also write the edits as VCF to this file."""
+    status: also write the status runs as BED to this file; vcf: also write the edits as VCF to this file; depth_bedgraph: also write
+    the depth runs as bedGraph to this file."""
     L = lib()
     L.pp_filter_polish_files_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int] + [C.c_char_p] * 6 + [
         C.c_double, C.c_double, C.POINTER(PolishParams), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
@@ -906,6 +948,7 @@ def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientat
         ctxs[0].set_changes_file(changes)
         ctxs[0].set_status_file(status)
         ctxs[0].set_vcf_file(vcf)
+        ctxs[0].set_depth_file(depth_bedgraph)
         try:
             rc = L.pp_filter_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), str(in1).encode(), str(in2).encode(),
                                                 str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
@@ -914,6 +957,7 @@ def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientat
             ctxs[0].set_changes_file(None)
             ctxs[0].set_status_file(None)
             ctxs[0].set_vcf_file(None)
+            ctxs[0].set_depth_file(None)
         if rc != PP_OK:
             raise ctxs[0]._err(rc)
         data = C.string_at(out, n.value)

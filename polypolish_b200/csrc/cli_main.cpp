@@ -9,7 +9,8 @@
 // GPUs filters a byte range of both SAM files; `filter` and `filter-polish` keep rejecting --gpus, as they always have), --quiet, --host-parse (polish: parse the
 // SAM text on the host instead of on the device; same output), --changes F (polish, filter-polish: the --debug rows of the changed
 // positions only), --status-bed F (polish, filter-polish: every position's --debug status as BED runs), --vcf F (polish,
-// filter-polish: the polish's edits to the draft as VCF records that rebuild the polished FASTA).
+// filter-polish: the polish's edits to the draft as VCF records that rebuild the polished FASTA), --depth-bedgraph F (polish,
+// filter-polish: every position's --debug depth as bedGraph runs).
 // All compute happens in libpolypolish_b200.so on the GPU.
 #include <cstdio>
 #include <unistd.h>
@@ -92,7 +93,8 @@ static void help_polish() {               // main.rs:77-108
     puts("          Print version");
     puts("\nH100 build, additive options: --device <N> (first GPU, default 0), --gpus <N> (contigs shard over N GPUs), --quiet, --host-parse, "
          "--changes <FILE> (the --debug rows of the changed positions only), --status-bed <FILE> (every position's --debug status as BED runs), "
-         "--vcf <FILE> (the edits to the draft as VCF records that rebuild the polished FASTA)");
+         "--vcf <FILE> (the edits to the draft as VCF records that rebuild the polished FASTA), "
+         "--depth-bedgraph <FILE> (every position's --debug depth as bedGraph runs)");
 }
 
 // clap accepts `--name=value`, `-m5` / `-m=5` and a `--` separator (everything after it is positional): normalise those forms
@@ -164,7 +166,7 @@ struct Args {
     std::vector<Token> tok;
     size_t i = 0;
     pp_polish_params prm{0.2, 0.5, 10, 5, 0};
-    std::string debug, changes, status_bed, vcf, in1, in2, out1, out2, orientation = "auto";
+    std::string debug, changes, status_bed, vcf, depth_bedgraph, in1, in2, out1, out2, orientation = "auto";
     double low = 0.1, high = 99.9;
     int device = 0, gpus = 1;
     bool quiet = false, host_parse = false;
@@ -175,11 +177,12 @@ struct Args {
     }
 };
 
-// -i / -v / -m / -d / --careful / --changes / --status-bed / --vcf of `polish` and `filter-polish`
+// -i / -v / -m / -d / --careful / --changes / --status-bed / --vcf / --depth-bedgraph of `polish` and `filter-polish`
 static bool polish_option(const std::string& a, Args& g) {
     if (a == "--changes") g.changes = g.value("--changes <FILE>");
     else if (a == "--status-bed") g.status_bed = g.value("--status-bed <FILE>");
     else if (a == "--vcf") g.vcf = g.value("--vcf <FILE>");
+    else if (a == "--depth-bedgraph") g.depth_bedgraph = g.value("--depth-bedgraph <FILE>");
     else if (a == "-i" || a == "--fraction_invalid") g.prm.fraction_invalid = parse_f64("--fraction_invalid <FRACTION_INVALID>", g.value("--fraction_invalid"));
     else if (a == "-v" || a == "--fraction_valid") g.prm.fraction_valid = parse_f64("--fraction_valid <FRACTION_VALID>", g.value("--fraction_valid"));
     else if (a == "-m" || a == "--max_errors") g.prm.max_errors = parse_u32("--max_errors <MAX_ERRORS>", g.value("--max_errors"));
@@ -242,6 +245,7 @@ static std::vector<pp_ctx*> open_contexts(const Args& g) {
     if (!g.changes.empty()) pp_set_changes_file(ctxs[0], g.changes.c_str());
     if (!g.status_bed.empty()) pp_set_status_file(ctxs[0], g.status_bed.c_str());
     if (!g.vcf.empty()) pp_set_vcf_file(ctxs[0], g.vcf.c_str());
+    if (!g.depth_bedgraph.empty()) pp_set_depth_file(ctxs[0], g.depth_bedgraph.c_str());
     return ctxs;
 }
 

@@ -3,6 +3,7 @@
 // so that the emulated change rows are checked byte for byte against the reference's.
 #pragma once
 #include <algorithm>
+#include <charconv>
 #include <cstdint>
 #include <cstdio>
 #include <string>
@@ -13,6 +14,16 @@
 namespace pp {
 
 inline const char* const DEBUG_HEADER = "name\tpos\tbase\tdepth\tinvalid\tvalid\tpileup\tstatus\tnew_base\n";
+
+// The --debug depth column's text ("%.1f" of the depth) of a depth printed as `tenths` tenths (depth_tenths in polish_dev.cuh), with
+// no floating point: tenths / 10, ".", tenths % 10.
+inline void depth_text(std::string& buf, uint64_t tenths) {
+    char t[24];
+    char* e = std::to_chars(t, t + sizeof t, tenths / 10).ptr;
+    *e++ = '.';
+    *e++ = (char)('0' + tenths % 10);
+    buf.append(t, e);
+}
 
 inline uint32_t get_u32(const uint8_t* p) { return p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
 

@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <algorithm>
+#include <charconv>
 #include <memory>
 #include <string>
 #include <string_view>
@@ -228,7 +229,8 @@ using FastaPtr = std::unique_ptr<pp_fasta, Deleter<pp_fasta_free>>;
 using PackPtr = std::unique_ptr<pp_pack, Deleter<pp_pack_free>>;
 using ShardsPtr = std::unique_ptr<pp_shards, Deleter<pp_shards_free>>;
 
-// --debug / --changes / --status-bed: the contexts record per-position data (Set = pp_polish_set_debug / pp_polish_set_changes / pp_polish_set_status) for the length of
+// --debug / --changes / --status-bed / --depth-bedgraph: the contexts record per-position data (Set = pp_polish_set_debug /
+// pp_polish_set_changes / pp_polish_set_status / pp_polish_set_depth) for the length of
 // the call.  They are left in mode 2 (not recording, the records of this call readable) when the call succeeded, otherwise in mode
 // 0, so that later calls neither record nor read stale data.
 template <int (*Set)(pp_ctx*, int)>
@@ -634,38 +636,47 @@ static int write_vcf(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs,
     return fwrite(buf.data(), 1, buf.size(), f) == buf.size() ? PP_OK : PP_ERR_IO;
 }
 
-// --status-bed: the status runs as BED lines, contigs in the input FASTA's order.  Every job reports the runs of its own contigs
-// (pp_polish_status_fetch); a run never crosses a contig, so each contig's lines are its runs in order.  PP_ERR_IO: the file could not
-// be written; another error: its message is on ctx.
-static int write_status_bed(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>& jobs, FILE* f) {
-    static const char* const word[6] = {"low_depth", "none", "multiple", "too_close", "kept", "changed"};
-    struct Run { uint64_t start, end; uint8_t status; };
+// --status-bed / --depth-bedgraph: the runs of a per-position report (Fetch = pp_polish_status_fetch / pp_polish_depth_fetch) as
+// "<contig>\t<start>\t<end>\t<value>" lines, the value written by Text, contigs in the input FASTA's order.  Every job reports the runs
+// of its own contigs; a run never crosses a contig, so each contig's lines are its runs in order.  PP_ERR_IO: the file could not be
+// written; another error: its message is on ctx.
+template <class T, int (*Fetch)(pp_ctx*, uint64_t, uint64_t*, T*, uint64_t*), void (*Text)(std::string&, T)>
+static int write_runs(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>& jobs, FILE* f) {
+    struct Run { uint64_t start, end; T value; };
     std::vector<std::vector<Run>> by_contig(contigs.n_contigs);
     for (const ShardJob& j : jobs) {
         uint64_t n = 0;
-        int rc = pp_polish_status_fetch(j.ctx, 0, nullptr, nullptr, &n);
+        int rc = Fetch(j.ctx, 0, nullptr, nullptr, &n);
         std::vector<uint64_t> start(n);
-        std::vector<uint8_t> status(n);
-        if (rc == PP_OK && n) rc = pp_polish_status_fetch(j.ctx, n, start.data(), status.data(), &n);
+        std::vector<T> value(n);
+        if (rc == PP_OK && n) rc = Fetch(j.ctx, n, start.data(), value.data(), &n);
         if (rc != PP_OK) return pp_ctx_fail(ctx, rc, std::string(pp_last_error(j.ctx)).c_str());
         const uint64_t G = j.contigs.off[j.contigs.n_contigs];
         for (uint64_t i = 0; i < n; ++i) {
             const auto cp = input_position(j, jobs.size() == 1, start[i]);
             const uint64_t end = i + 1 < n ? start[i + 1] : G;
-            by_contig[cp.first].push_back({cp.second, cp.second + (end - start[i]), status[i]});
+            by_contig[cp.first].push_back({cp.second, cp.second + (end - start[i]), value[i]});
         }
     }
     std::string buf;
-    char tmp[64];
+    char num[24];
     for (uint32_t c = 0; c < contigs.n_contigs; ++c) {
         const char* name = pp_fasta_name(fa, c);
-        for (const Run& r : by_contig[c]) {
-            snprintf(tmp, sizeof tmp, "\t%llu\t%llu\t", (unsigned long long)r.start, (unsigned long long)r.end);
-            buf += name; buf += tmp; buf += word[r.status < 6 ? r.status : 0]; buf += '\n';
+        for (const Run& r : by_contig[c]) {          // (millions of lines for the depth runs: no snprintf)
+            buf += name; buf += '\t';
+            buf.append(num, std::to_chars(num, num + sizeof num, r.start).ptr); buf += '\t';
+            buf.append(num, std::to_chars(num, num + sizeof num, r.end).ptr); buf += '\t';
+            Text(buf, r.value); buf += '\n';
         }
     }
     return fwrite(buf.data(), 1, buf.size(), f) == buf.size() ? PP_OK : PP_ERR_IO;
 }
+static void status_text(std::string& buf, uint8_t status) {
+    static const char* const word[6] = {"low_depth", "none", "multiple", "too_close", "kept", "changed"};
+    buf += word[status < 6 ? status : 0];
+}
+static constexpr auto write_status_bed = write_runs<uint8_t, pp_polish_status_fetch, status_text>;
+static constexpr auto write_depth_bedgraph = write_runs<uint64_t, pp_polish_depth_fetch, pp::depth_text>;
 
 static void print_timing(const Load& ld) {
     fputs(ld.timing.c_str(), stderr);
@@ -696,11 +707,12 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     for (int i = 0; i < n_sams; ++i)
         if (!pp::file_exists(sams[i])) return pp_ctx_fail(ctx, PP_ERR_INPUT, ("\"" + std::string(sams[i]) + "\" file does not exist").c_str());
     const bool debug = debug_path && debug_path[0];
-    const std::string changes_path = pp_ctx_changes_file(ctx), status_path = pp_ctx_status_file(ctx), vcf_path = pp_ctx_vcf_file(ctx);
-    const bool changes = !changes_path.empty(), status = !status_path.empty(), vcf = !vcf_path.empty();
-    FILE *debug_file = nullptr, *changes_file = nullptr, *status_file = nullptr, *vcf_file = nullptr;
+    const std::string changes_path = pp_ctx_changes_file(ctx), status_path = pp_ctx_status_file(ctx), vcf_path = pp_ctx_vcf_file(ctx),
+                      depth_path = pp_ctx_depth_file(ctx);
+    const bool changes = !changes_path.empty(), status = !status_path.empty(), vcf = !vcf_path.empty(), depth = !depth_path.empty();
+    FILE *debug_file = nullptr, *changes_file = nullptr, *status_file = nullptr, *vcf_file = nullptr, *depth_file = nullptr;
     struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file}, closer2{changes_file}, closer3{status_file},
-        closer4{vcf_file};
+        closer4{vcf_file}, closer5{depth_file};
     // create_debug_file polish.rs:230-244; the other reports are worded like it
     auto create = [ctx](const std::string& path, FILE*& file) {
         file = fopen(path.c_str(), "wb");
@@ -710,10 +722,12 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     if (created == PP_OK && changes) created = create(changes_path, changes_file);
     if (created == PP_OK && status) created = create(status_path, status_file);
     if (created == PP_OK && vcf) created = create(vcf_path, vcf_file);
+    if (created == PP_OK && depth) created = create(depth_path, depth_file);
     if (created != PP_OK) return created;
     Recording<pp_polish_set_debug> recording(&ctx, 1, debug);
     Recording<pp_polish_set_changes> recording_changes(ctxs, n_ctx, changes || vcf);
     Recording<pp_polish_set_status> recording_status(ctxs, n_ctx, status);
+    Recording<pp_polish_set_depth> recording_depth(ctxs, n_ctx, depth);
 
     // the first SAM file starts streaming into HBM while the assembly is loaded
     const bool device_parser = pp_get_parser(ctx) == 0;
@@ -776,8 +790,12 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
         rc = write_vcf(ctx, fa.get(), contigs, change_rows, vcf_file);
         if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + vcf_path + "\"").c_str());
     }
+    if (rc == PP_OK && depth) {
+        rc = write_depth_bedgraph(ctx, fa.get(), contigs, ld.jobs, depth_file);
+        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + depth_path + "\"").c_str());
+    }
     if (rc != PP_OK) return rc;
-    recording.ok = recording_changes.ok = recording_status.ok = true;
+    recording.ok = recording_changes.ok = recording_status.ok = recording_depth.ok = true;
     if (verbose) {
         uint64_t n_used = 0;
         for (const ShardJob& j : ld.jobs) n_used += j.res.n_aln_used;

@@ -47,6 +47,9 @@
 #define TL_FAST_LEN 192              // longest read the register-resident fast path takes
 #define PR_THREADS 256               // k_prep CTA: one alignment per thread
 #define SC_GROUP_SCAN_LIMIT 8192     // alignments of one read group a thread will scan outside its block for k
+#define SR_THREADS 256               // k_status_heads / k_status_runs: positions per CTA = SR_CHUNK
+#define SR_PER_THREAD 16
+#define SR_CHUNK (SR_THREADS * SR_PER_THREAD)
 #define VT_THREADS 256
 #define VT_ITEMS 8
 #define VT_CHUNK (VT_THREADS * VT_ITEMS)
@@ -184,6 +187,7 @@ static inline double emu_ull2double(unsigned long long x, bool up) {
 static inline double __ull2double_rd(unsigned long long x) { return emu_ull2double(x, false); }
 static inline double __ull2double_ru(unsigned long long x) { return emu_ull2double(x, true); }
 static inline double __ull2double_rn(unsigned long long x) { return (double)x; }
+static inline double __fma_rn(double a, double b, double c) { return std::fma(a, b, c); }
 // Reads the chunk loop handed to the general walk from the pool (queued, or walked in place when the queue is full), summed over
 // the tiles that look at them: the emulator's tests read the exported symbol to see how many reads the staged walk left behind.
 inline std::atomic<unsigned long long> emu_n_queued{0};
@@ -326,6 +330,22 @@ __device__ __forceinline__ DepthBounds depth_bounds(uint32_t cover, unsigned lon
 }
 __device__ __forceinline__ unsigned long long depth_deficit(uint32_t k) {   // 2^40 - round(2^40 / k), k >= 2
     return (1ull << 40) - ((1ull << 40) + k / 2) / k;
+}
+
+// What "%.1f" prints for a non-negative finite depth x (the --debug depth column, debug_rows.h), times ten, without formatting: the
+// exact binary value of x rounded to a tenth, an exact tie to the even tenth.  q = rint(fl(10 x)) is within one of the answer
+// (|fl(10 x) - 10 x| < 1/2 below 2^49).  The answer is q + 1 where 20 x > 2q + 1, q - 1 where 20 x < 2q - 1, else q, and the tie
+// 20 x = 2q +- 1 goes to the even neighbour.  FMA rounds x * 20 - (2q +- 1) once, so its sign is the exact difference's, and zero
+// only when that is zero (2q +- 1 < 2^37 is exact).  Monotone in x, like every rounding.
+__device__ __forceinline__ unsigned long long depth_tenths(double x) {
+    const double q = rint(__dmul_rn(x, 10.0));
+    const double up = __fma_rn(x, 20.0, -(2.0 * q + 1.0)), dn = __fma_rn(x, 20.0, -(2.0 * q - 1.0));
+    const unsigned long long u = (unsigned long long)q;
+    if (up > 0.0) return u + 1;
+    if (up == 0.0) return u + (u & 1ull);
+    if (dn < 0.0) return u - 1;
+    if (dn == 0.0) return u - (u & 1ull);
+    return u;
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -697,8 +717,14 @@ struct VoteParams {
     uint32_t chg_cap;
     // --status-bed: one byte per position (padded to whole SR_CHUNKs), bits 0..2 the BaseStatus as pp_debug_pos.status, bit 7 set where
     // a contig starts; k_status_runs turns it into runs.  Read only by k_tile's status mode.
+    // --depth-bedgraph: in depth mode the same pointer is first one 8-byte key per position (depth_key_bytes, padded the same way), bits
+    // 0..62 the printed depth in tenths (depth_tenths; < 2^36 at any 32-bit cover), bit 63 set where a contig starts, and the status
+    // bytes follow the keys.  (One pointer for both reports: a larger parameter block changed the register allocation of the
+    // instances that record nothing.)
     uint8_t* sts;
 };
+// bytes of depth mode's keys at the start of VoteParams::sts
+__host__ __device__ __forceinline__ size_t depth_key_bytes(uint64_t G) { return (size_t)((G + SR_CHUNK - 1) / SR_CHUNK) * SR_CHUNK * 8; }
 
 // What the other-allele slow path needs, passed by value so that the kernel parameter structs are never
 // spilled to local memory for a call.
@@ -1442,9 +1468,10 @@ __device__ __forceinline__ void depth_walk(const DevData& d, TileShared& sh, Wal
 }
 
 // CHG: the change report is recorded (vp.chg; without it the vp.chg* fields are not read).  STS: every position's status is
-// recorded (vp.sts).  Template arguments, so that the kernel without a report does the work it did before the reports existed (as a
-// run-time test CHG measured up to 0.5 % slower on an H100, 700 W, 5 Mbp x 100x).
-template <int BITS, bool CHG = false, bool STS = false>
+// recorded (vp.sts).  DEP: every position's printed depth is recorded (vp.sts, keys first).  Template arguments, so that the kernel
+// without a report does the work it did before the reports existed (as a run-time test CHG measured up to 0.5 % slower on an H100,
+// 700 W, 5 Mbp x 100x).
+template <int BITS, bool CHG = false, bool STS = false, bool DEP = false>
 __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp, TileShared& sh) {
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const DevParams prm = *d.prm;
@@ -1681,6 +1708,9 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
         // there a sub-tile also walks when one of its positions passes these tests, which every position that reaches the vote does.
         // The status reads depth only through the thresholds (vote_thresholds): in status mode a sub-tile also walks when a position
         // with k != 1 coverage gets other thresholds at the two ends of its bound, whatever the tests say of the emitted base.
+        // The depth report prints depth to a tenth: in depth mode a sub-tile also walks when a position with k != 1 coverage prints
+        // differently at the two ends of its bound.  Printing is monotone, so where both ends print the same the reference's sum,
+        // which lies between them, prints that too, and the lower end is recorded.
         bool walk;
         {
             bool open = false;
@@ -1693,6 +1723,10 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                     if (STS) {
                         const DepthBounds db = depth_bounds(cover[i], sh.deficit[rel]);
                         if (!same_thresholds(prm, db.lo, db.hi)) { open = true; continue; }
+                    }
+                    if (DEP) {
+                        const DepthBounds db = depth_bounds(cover[i], sh.deficit[rel]);
+                        if (depth_tenths(db.lo) != depth_tenths(db.hi)) { open = true; continue; }
                     }
                     const uint32_t mx = max(max(max(sh.ex[0][rel], sh.ex[1][rel]), max(sh.ex[2][rel], sh.ex[3][rel])), max(sh.del[rel], sh.oth[rel]));
                     if (mx == 0 || mx < prm.min_depth) continue;
@@ -1724,8 +1758,9 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             ctg = clo;
         }
         uint32_t next_start = (ctg + 1 < d.n_contigs) ? (uint32_t)d.contig_off[ctg + 1] : 0xFFFFFFFFu;
-        uint32_t sts4 = 0, ctg_start = 0;                  // status mode: the four status bytes; the start of contig ctg
-        if constexpr (STS) ctg_start = (p0 < d.G) ? (uint32_t)d.contig_off[ctg] : 0u;
+        uint32_t sts4 = 0, ctg_start = 0;                  // status mode: the four status bytes; status / depth mode: the start of contig ctg
+        unsigned long long dep4[TL_PER_THREAD] = {0, 0, 0, 0};     // depth mode: the four keys
+        if constexpr (STS || DEP) ctg_start = (p0 < d.G) ? (uint32_t)d.contig_off[ctg] : 0u;
         const uint32_t dr = *reinterpret_cast<const uint32_t*>(d.draft + p0);      // draft is padded past G
 #pragma unroll
         for (int i = 0; i < TL_PER_THREAD; ++i) {
@@ -1739,12 +1774,13 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 n_changed = n_zero = 0;
                 tdepth = 0.0;
                 ctg++;
-                if constexpr (STS) ctg_start = next_start;
+                if constexpr (STS || DEP) ctg_start = next_start;
                 next_start = (ctg + 1 < d.n_contigs) ? (uint32_t)d.contig_off[ctg + 1] : 0xFFFFFFFFu;
             }
             const uint32_t orig = (dr >> (i * 8)) & 255u;
             const uint32_t cov = cover[i];
             if constexpr (STS) if (p == ctg_start) sts4 |= 0x80u << (8 * i);
+            if constexpr (DEP) if (p == ctg_start) dep4[i] = 1ull << 63;
             if (cov == 0) {                                    // depth 0: always the original base
                 n_zero++;
                 po[i].packed = (orig == '-' ? 0u : 1u) | (orig << 16);
@@ -1769,6 +1805,9 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
                 else { const DepthBounds db = depth_bounds(cov, sh.deficit[rel]); depth = db.fx; vdepth = db.lo; }
             }
             tdepth += depth;
+            // depth mode: the printed depth, from the reference's sum where the warp walked, else from the lower bound, whose print
+            // phase D found to be the reference's; without k != 1 coverage the depth is cover, exactly
+            if constexpr (DEP) dep4[i] |= ((multi >> i) & 1u) ? depth_tenths(vdepth) : 10ull * cov;
             uint32_t cA = sh.ex[0][rel], cC = sh.ex[1][rel], cG = sh.ex[2][rel], cT = sh.ex[3][rel];
             const uint32_t cDel = sh.del[rel], n_other = sh.oth[rel];
             // (status mode: every covered position votes, its status being what the shortcuts below do not decide)
@@ -1801,7 +1840,12 @@ __device__ __forceinline__ void tile_body(const DevData& d, const VoteParams& vp
             tlen += po[i].packed & 0xFFFFu;
             if constexpr (STS) sts4 |= ((po[i].packed >> 26) & 7u) << (8 * i);
         }
-        if constexpr (STS) *reinterpret_cast<uint32_t*>(vp.sts + p0) = sts4;
+        if constexpr (STS) *reinterpret_cast<uint32_t*>(vp.sts + (DEP ? depth_key_bytes(d.G) : 0) + p0) = sts4;
+        if constexpr (DEP) {
+            ulonglong2* const key = reinterpret_cast<ulonglong2*>(vp.sts) + p0 / 2;
+            key[0] = make_ulonglong2(dep4[0], dep4[1]);
+            key[1] = make_ulonglong2(dep4[2], dep4[3]);
+        }
         {   // per-contig statistics: one atomic per warp when the whole warp sits in one contig (nearly always)
             const uint32_t ctg0 = __shfl_sync(0xffffffffu, ctg, 0);
             if (__ballot_sync(0xffffffffu, ctg != ctg0) == 0u) {
@@ -1856,75 +1900,93 @@ static_assert(TL_PER_THREAD == 4, "the verdict store packs four positions per th
 #if !defined(PP_EMULATE)
 // One CTA per SM: built for sm_90a, the body needs ~100 registers per thread.  Capped at 64 for two CTAs per SM it spills, and on an
 // H100 (400 W) the tile kernel took 0.79 ms per 5 Mbp x 100x call that way against 0.71 ms with one CTA per SM.
-template <int BITS, bool CHG, bool STS>
+template <int BITS, bool CHG, bool STS, bool DEP>
 __global__ void __launch_bounds__(TL_THREADS, 1) k_tile(DevData d, VoteParams vp) {
     extern __shared__ __align__(16) unsigned char tile_smem[];
-    tile_body<BITS, CHG, STS>(d, vp, *reinterpret_cast<TileShared*>(tile_smem));
+    tile_body<BITS, CHG, STS, DEP>(d, vp, *reinterpret_cast<TileShared*>(tile_smem));
 }
 #endif
 
 // ------------------------------------------------------------------------------------------------------
-// k_status_heads / k_status_runs: k_tile's status bytes (VoteParams::sts) -> runs of equal status.  Position p starts a run where a
-// contig starts or where its status differs from position p - 1's.  CTA b looks at positions [b, b + 1) * SR_CHUNK: the first kernel
-// counts its runs, an exclusive scan of the counts gives each CTA its first run (and the total, so that the run arrays are sized
-// exactly), the second writes (start, status) of its runs in position order.  The status array is padded to whole SR_CHUNKs.
+// k_status_heads / k_status_runs: a per-position report of k_tile -> runs of equal value.  T is the report's element: the status byte
+// (VoteParams::sts) or the depth key (the start of VoteParams::sts in depth mode); RunMark<T> says which bit marks a contig start
+// and which bits are the value.
+// Position p starts a run where a contig starts or where its value differs from position p - 1's.  CTA b looks at positions
+// [b, b + 1) * SR_CHUNK: the first kernel counts its runs, an exclusive scan of the counts gives each CTA its first run (and the total,
+// so that the run arrays are sized exactly), the second writes (start, value) of its runs in position order.  The report is padded to
+// whole SR_CHUNKs.
 // ------------------------------------------------------------------------------------------------------
-#define SR_THREADS 256
-#define SR_PER_THREAD 16
-#define SR_CHUNK (SR_THREADS * SR_PER_THREAD)
-static_assert(SR_CHUNK % TL_T == 0, "the status array padded to whole SR_CHUNKs also holds k_tile's whole tiles");
+static_assert(SR_CHUNK % TL_T == 0, "a report padded to whole SR_CHUNKs also holds k_tile's whole tiles");
 struct RunShared {
     unsigned long long s_warp[SR_THREADS / 32];
     unsigned long long s_total;
 };
 
-// bit i: position p0 + i (< G) starts a run; *w receives the sixteen status bytes
-__device__ __forceinline__ uint32_t status_heads(const uint8_t* sts, uint32_t G, uint32_t p0, uint32_t w[4]) {
+template <class T> struct RunMark;
+template <> struct RunMark<uint8_t> { static constexpr uint8_t head = 0x80u, value = 7u; };
+template <> struct RunMark<unsigned long long> { static constexpr unsigned long long head = 1ull << 63, value = ~(1ull << 63); };
+
+// element i of the sixteen that status_heads loaded into w
+template <class T> __device__ __forceinline__ T run_elem(const uint32_t* w, int i) {
+    if constexpr (sizeof(T) == 1) return (T)((w[i >> 2] >> (8 * (i & 3))) & 255u);
+    else return (T)w[2 * i] | (T)w[2 * i + 1] << 32;
+}
+
+// bit i: position p0 + i (< G) starts a run; w receives the sixteen elements
+template <class T>
+__device__ __forceinline__ uint32_t status_heads(const T* e, uint32_t G, uint32_t p0, uint32_t w[4 * sizeof(T)]) {
+    static_assert(sizeof(T) == 1 || sizeof(T) == 8, "a status byte or a depth key");
     if (p0 >= G) return 0;
-    const uint4 q = *reinterpret_cast<const uint4*>(sts + p0);
-    w[0] = q.x; w[1] = q.y; w[2] = q.z; w[3] = q.w;
-    uint32_t prev = p0 ? sts[p0 - 1] : 0u;                   // (position 0 starts contig 0: its byte has bit 7)
+#pragma unroll
+    for (int j = 0; j < (int)sizeof(T); ++j) {
+        const uint4 q = reinterpret_cast<const uint4*>(e + p0)[j];
+        w[4 * j] = q.x; w[4 * j + 1] = q.y; w[4 * j + 2] = q.z; w[4 * j + 3] = q.w;
+    }
+    T prev = p0 ? e[p0 - 1] : T(0);                          // (position 0 starts contig 0: its element has the head bit)
     uint32_t m = 0;
 #pragma unroll
     for (int i = 0; i < SR_PER_THREAD; ++i) {
-        const uint32_t s = (w[i >> 2] >> (8 * (i & 3))) & 255u;
-        if (p0 + i < G && ((s & 0x80u) || ((s ^ prev) & 7u))) m |= 1u << i;
+        const T s = run_elem<T>(w, i);
+        if (p0 + i < G && ((s & RunMark<T>::head) || ((s ^ prev) & RunMark<T>::value))) m |= 1u << i;
         prev = s;
     }
     return m;
 }
 
-__device__ __forceinline__ void status_heads_body(const uint8_t* sts, uint32_t G, uint32_t* count, RunShared& sh) {
-    uint32_t w[4];
-    const uint32_t m = status_heads(sts, G, blockIdx.x * SR_CHUNK + threadIdx.x * SR_PER_THREAD, w);
+template <class T>
+__device__ __forceinline__ void status_heads_body(const T* e, uint32_t G, uint32_t* count, RunShared& sh) {
+    uint32_t w[4 * sizeof(T)];
+    const uint32_t m = status_heads(e, G, blockIdx.x * SR_CHUNK + threadIdx.x * SR_PER_THREAD, w);
     block_exscan<SR_THREADS>((unsigned long long)__popc(m), sh.s_warp, &sh.s_total);
     if (threadIdx.x == 0) count[blockIdx.x] = (uint32_t)sh.s_total;
 }
 
-// first[b]: the exclusive scan of the counts
-__device__ __forceinline__ void status_runs_body(const uint8_t* sts, uint32_t G, const uint32_t* first, uint32_t* start, uint8_t* status,
-                                                 RunShared& sh) {
-    uint32_t w[4];
+// first[b]: the exclusive scan of the counts; value[o]: the run's element without the head bit
+template <class T>
+__device__ __forceinline__ void status_runs_body(const T* e, uint32_t G, const uint32_t* first, uint32_t* start, T* value, RunShared& sh) {
+    uint32_t w[4 * sizeof(T)];
     const uint32_t p0 = blockIdx.x * SR_CHUNK + threadIdx.x * SR_PER_THREAD;
-    uint32_t m = status_heads(sts, G, p0, w);
+    uint32_t m = status_heads(e, G, p0, w);
     uint32_t o = first[blockIdx.x] + (uint32_t)block_exscan<SR_THREADS>((unsigned long long)__popc(m), sh.s_warp, &sh.s_total);
     while (m) {
         const int i = __ffs(m) - 1;
         m &= m - 1;
         start[o] = p0 + i;
-        status[o] = (uint8_t)((w[i >> 2] >> (8 * (i & 3))) & 7u);
+        value[o] = (T)(run_elem<T>(w, i) & RunMark<T>::value);
         o++;
     }
 }
 
 #if !defined(PP_EMULATE)
-__global__ void __launch_bounds__(SR_THREADS) k_status_heads(const uint8_t* sts, uint32_t G, uint32_t* count) {
+template <class T>
+__global__ void __launch_bounds__(SR_THREADS) k_status_heads(const T* e, uint32_t G, uint32_t* count) {
     __shared__ RunShared sh;
-    status_heads_body(sts, G, count, sh);
+    status_heads_body(e, G, count, sh);
 }
-__global__ void __launch_bounds__(SR_THREADS) k_status_runs(const uint8_t* sts, uint32_t G, const uint32_t* first, uint32_t* start, uint8_t* status) {
+template <class T>
+__global__ void __launch_bounds__(SR_THREADS) k_status_runs(const T* e, uint32_t G, const uint32_t* first, uint32_t* start, T* value) {
     __shared__ RunShared sh;
-    status_runs_body(sts, G, first, start, status, sh);
+    status_runs_body(e, G, first, start, value, sh);
 }
 #endif
 

@@ -376,17 +376,19 @@ static const char* err_text(unsigned code) {
     }
 }
 
-// --status-bed: k_tile's status bytes, padded to whole CTAs of k_status_heads / k_status_runs (which load 16 bytes per thread)
+// --status-bed: k_tile's status bytes, padded to whole CTAs of k_status_heads / k_status_runs (which load 16 elements per thread); the
+// depth keys are padded the same way (depth_key_bytes)
 static size_t status_bytes(uint64_t G) { return (size_t)((G + SR_CHUNK - 1) / SR_CHUNK) * SR_CHUNK + 16; }
 
-// The status bytes of a call -> its runs in B_RUNSTART / B_RUNSTS, sized from the count (ctx->n_runs).
-static int status_runs(pp_ctx* ctx, const uint8_t* sts) {
+// A call's status bytes or depth keys -> its runs in b[b_start] / b[b_value], sized from the count (*n_runs).
+template <class T>
+static int report_runs(pp_ctx* ctx, const T* e, int b_start, int b_value, uint32_t* n_runs) {
     cudaStream_t s = ctx->stream;
     const uint32_t G = (uint32_t)ctx->G, n_blk = (uint32_t)((ctx->G + SR_CHUNK - 1) / SR_CHUNK);
     CK(ctx->b[B_RUNFIRST].ensure(((size_t)n_blk + 1) * 4));
     uint32_t* first = ctx->b[B_RUNFIRST].as<uint32_t>();
     CK(cudaMemsetAsync(first + n_blk, 0, 4, s));
-    if (n_blk) k_status_heads<<<n_blk, SR_THREADS, 0, s>>>(sts, G, first);
+    if (n_blk) k_status_heads<T><<<n_blk, SR_THREADS, 0, s>>>(e, G, first);
     size_t tb = 0;
     CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, first, first, (int)n_blk + 1, s));
     CK(ctx->b[B_CUBTMP].ensure(tb + 256));
@@ -396,13 +398,21 @@ static int status_runs(pp_ctx* ctx, const uint8_t* sts) {
     CK(cudaMemcpyAsync(&n, first + n_blk, 4, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     CK(cudaGetLastError());
-    CK(ctx->b[B_RUNSTART].ensure((size_t)n * 4 + 4)); CK(ctx->b[B_RUNSTS].ensure((size_t)n + 4));
-    if (n_blk) k_status_runs<<<n_blk, SR_THREADS, 0, s>>>(sts, G, first, ctx->b[B_RUNSTART].as<uint32_t>(), ctx->b[B_RUNSTS].as<uint8_t>());
+    CK(ctx->b[b_start].ensure((size_t)n * 4 + 4)); CK(ctx->b[b_value].ensure((size_t)n * sizeof(T) + 8));
+    if (n_blk) k_status_runs<T><<<n_blk, SR_THREADS, 0, s>>>(e, G, first, ctx->b[b_start].as<uint32_t>(), ctx->b[b_value].as<T>());
     CK(cudaGetLastError());
     ctx->launches += 2;
-    ctx->n_runs = n;
-    ctx->have_status = true;
+    *n_runs = n;
     return PP_OK;
+}
+
+// The k_tile instance that records what is asked for (CHG change list, STS status bytes, DEP depth keys).
+using TileKernel = void (*)(DevData, VoteParams);
+template <int BITS> static TileKernel tile_kernel(bool chg, bool sts, bool dep) {
+    static const TileKernel k[8] = {k_tile<BITS, false, false, false>, k_tile<BITS, false, false, true>, k_tile<BITS, false, true, false>,
+                                    k_tile<BITS, false, true, true>, k_tile<BITS, true, false, false>, k_tile<BITS, true, false, true>,
+                                    k_tile<BITS, true, true, false>, k_tile<BITS, true, true, true>};
+    return k[(chg ? 4 : 0) + (sts ? 2 : 0) + (dep ? 1 : 0)];
 }
 
 template <int BITS>
@@ -411,20 +421,16 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
     const uint64_t G = ctx->G, n_aln = ctx->n_aln;
     const uint32_t n_tiles = (uint32_t)((G + TL_T - 1) / TL_T);              // = vote / compaction chunks
     const size_t padG = (size_t)n_tiles * TL_T + 16;                          // k_tile / k_compact move whole chunks with vector accesses
-    ctx->have_changes = ctx->have_status = false;
+    ctx->have_changes = ctx->have_status = ctx->have_depth = false;
 
     CK(ctx->b[B_OUTOFF].ensure(((size_t)ctx->n_contigs + 1) * 8));
     CK(ctx->b[B_RES].ensure(padG * 2)); CK(ctx->b[B_RECAT].ensure((G + 1) * 4)); CK(ctx->b[B_CHUNKDELTA].ensure((size_t)n_tiles * 8));
     CK(ctx->b[B_PARAMS].ensure(sizeof(DevParams)));
     if (!ctx->tile_attr_set) {
-        CK(cudaFuncSetAttribute(k_tile<4, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<8, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<8, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<4, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<8, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<4, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
-        CK(cudaFuncSetAttribute(k_tile<8, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        for (int i = 0; i < 8; ++i) {
+            CK(cudaFuncSetAttribute(tile_kernel<4>(i & 4, i & 2, i & 1), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+            CK(cudaFuncSetAttribute(tile_kernel<8>(i & 4, i & 2, i & 1), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileShared)));
+        }
         ctx->tile_attr_set = true;
     }
 
@@ -448,6 +454,10 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
         uint8_t* zp = ctx->b[B_ZEROPOOL].as<uint8_t>();
         CK(ctx->b[B_NODES].ensure((size_t)node_cap * sizeof(OthNode)));
         CK(ctx->b[B_OUT].ensure(out_cap + 64));
+        // --depth-bedgraph / --status-bed: the depth keys, then the status bytes, in one buffer (VoteParams::sts), allocated before the
+        // timed stages
+        const size_t key_bytes = ctx->depth_on ? depth_key_bytes(G) : 0;
+        if (ctx->status_on || ctx->depth_on) CK(ctx->b[B_STS].ensure(key_bytes + (ctx->status_on ? status_bytes(G) : 16)));
 
         DevData d;
         fill_data(ctx, d);
@@ -500,11 +510,9 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
             CK(ctx->b[B_CHG].ensure((size_t)ctx->chg_cap * sizeof(pp_debug_pos))); CK(ctx->b[B_CHGPOS].ensure((size_t)ctx->chg_cap * 4));
             vp.chg = ctx->b[B_CHG].as<pp_debug_pos>(); vp.chg_pos = ctx->b[B_CHGPOS].as<uint32_t>(); vp.chg_cap = ctx->chg_cap;
         }
-        vp.sts = nullptr;
-        if (ctx->status_on) { CK(ctx->b[B_STS].ensure(status_bytes(G))); vp.sts = ctx->b[B_STS].as<uint8_t>(); }
+        vp.sts = (ctx->status_on || ctx->depth_on) ? ctx->b[B_STS].as<uint8_t>() : nullptr;
         {
-            auto kt = vp.chg ? (vp.sts ? k_tile<BITS, true, true> : k_tile<BITS, true, false>)
-                             : (vp.sts ? k_tile<BITS, false, true> : k_tile<BITS, false, false>);
+            const TileKernel kt = tile_kernel<BITS>(vp.chg, ctx->status_on, ctx->depth_on);
             int occ = 1;
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kt, TL_THREADS, sizeof(TileShared)));
             const uint32_t grid = std::min<uint32_t>(n_tiles, (uint32_t)ctx->sm_count * (uint32_t)std::max(occ, 1));   // persistent: tiles by ticket
@@ -550,8 +558,14 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
         ctx->have_debug = ctx->debug_on; ctx->last_head = d.oth_head; ctx->last_nodes = std::min(hs.node_count, node_cap);
         ctx->have_changes = ctx->changes_on; ctx->n_changes = ctx->changes_on ? hs.n_changes : 0; ctx->chg_pool = -1;
         if (ctx->status_on) {
-            const int rc = status_runs(ctx, vp.sts);
+            const int rc = report_runs(ctx, vp.sts + key_bytes, B_RUNSTART, B_RUNSTS, &ctx->n_runs);
             if (rc != PP_OK) return rc;
+            ctx->have_status = true;
+        }
+        if (ctx->depth_on) {
+            const int rc = report_runs(ctx, reinterpret_cast<const unsigned long long*>(vp.sts), B_DEPSTART, B_DEPRUN, &ctx->n_dep_runs);
+            if (rc != PP_OK) return rc;
+            ctx->have_depth = true;
         }
         res->out_len = hs.out_len;
         res->n_aln_used = hs.n_used;
@@ -776,6 +790,40 @@ extern "C" int pp_polish_status_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* s
     if (n) {
         CK(cudaMemcpyAsync(st.data(), ctx->b[B_RUNSTART].p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaMemcpyAsync(status, ctx->b[B_RUNSTS].p, n, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::copy(st.begin(), st.end(), start);
+    return PP_OK;
+}
+
+extern "C" int pp_polish_set_depth(pp_ctx* ctx, int on) {
+    if (!ctx) return PP_ERR_ARG;
+    ctx->depth_on = on == 1;            // 2 = stop recording but keep the last call's runs readable
+    if (on != 1) { CK(cudaSetDevice(ctx->device)); ctx->b[B_STS].release(); ctx->b[B_RUNFIRST].release(); }
+    if (on == 0) { ctx->have_depth = false; ctx->b[B_DEPSTART].release(); ctx->b[B_DEPRUN].release(); }
+    return PP_OK;
+}
+
+extern "C" int pp_set_depth_file(pp_ctx* ctx, const char* path) {
+    if (!ctx) return PP_ERR_ARG;
+    ctx->depth_path = path ? path : "";
+    return PP_OK;
+}
+const char* pp_ctx_depth_file(pp_ctx* ctx) { return ctx->depth_path.c_str(); }
+
+extern "C" int pp_polish_depth_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint64_t* tenths, uint64_t* n_runs) {
+    if (!ctx) return PP_ERR_ARG;
+    if (!ctx->have_depth) return ctx->fail(PP_ERR_ARG, "pp_polish_depth_fetch: the last polish did not record depth (pp_polish_set_depth)");
+    if (!n_runs) return ctx->fail(PP_ERR_ARG, "pp_polish_depth_fetch: null size pointer");
+    const uint32_t n = ctx->n_dep_runs;
+    *n_runs = n;
+    if (run_cap == 0 && n > 0) return PP_OK;                                                   // size query
+    if (run_cap < n || (n && (!start || !tenths))) return ctx->fail(PP_ERR_ARG, "pp_polish_depth_fetch: buffers too small");
+    CK(cudaSetDevice(ctx->device));
+    std::vector<uint32_t> st(n);
+    if (n) {
+        CK(cudaMemcpyAsync(st.data(), ctx->b[B_DEPSTART].p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(tenths, ctx->b[B_DEPRUN].p, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     }
     CK(cudaStreamSynchronize(ctx->stream));
     std::copy(st.begin(), st.end(), start);

@@ -32,6 +32,7 @@ enum { B_CONTIG, B_REFSTART, B_READID, B_SEQOFF, B_SEQLEN, B_CIGOFF, B_NCIG, B_N
        B_DRAFT, B_CTGOFF, B_ZEROPOOL, B_RECS, B_KEY, B_VAL, B_SKEY, B_SVAL, B_BINSTART, B_SREC, B_SSEQ, B_KF, B_NK, B_TILEORDER, B_ERRC, B_GQ, B_HEADS, B_NODES, B_CUBTMP, B_SEQ2, B_OUT,
        B_OUTOFF, B_DEBUG, B_RES, B_RECAT, B_CHUNKDELTA, B_PARAMS, B_SCRATCH, B_SCRATCH2,
        B_CHG, B_CHGPOS, B_STRPOS, B_STRPOOL, B_STROFF, B_STS, B_RUNFIRST, B_RUNSTART, B_RUNSTS,
+       B_DEPSTART, B_DEPRUN,
        B_TOKLINE, B_TOKTMP, B_TOKNAMES, B_COUNT };
 
 struct pp_ctx {
@@ -69,6 +70,10 @@ struct pp_ctx {
     bool status_on = false, have_status = false;
     uint32_t n_runs = 0;
     std::string status_path;              // pp_set_status_file: the BED the file-level commands also write
+    // --depth-bedgraph (pp_polish_set_depth): the depth runs of the last call (B_DEPSTART / B_DEPRUN, exactly n_dep_runs long)
+    bool depth_on = false, have_depth = false;
+    uint32_t n_dep_runs = 0;
+    std::string depth_path;               // pp_set_depth_file: the bedGraph the file-level commands also write
     std::string vcf_path;                 // pp_set_vcf_file: the VCF the file-level commands also write (from the change rows)
     TokState* tok = nullptr;              // SAM tokeniser state (tok_kernels.cu), created on first use
     int parser = 0;                       // pp_set_parser: 0 device tokeniser where possible, 1 host packer only

@@ -110,6 +110,8 @@ int pp_ctx_fail(pp_ctx* ctx, int code, const char* msg);
 const char* pp_ctx_changes_file(pp_ctx* ctx);
 // the BED path of pp_set_status_file ("" = none)
 const char* pp_ctx_status_file(pp_ctx* ctx);
+// the bedGraph path of pp_set_depth_file ("" = none)
+const char* pp_ctx_depth_file(pp_ctx* ctx);
 // the VCF path of pp_set_vcf_file ("" = none)
 const char* pp_ctx_vcf_file(pp_ctx* ctx);
 // --debug: the allele strings (k_allele_strings' format, row i at pool[off[i]]) of the last call's records at n global positions
