@@ -3,6 +3,7 @@
 Names follow the reference's command surface (main.rs:44-109): `polish(...)` and `filter_sams(...)` take the same
 options with the same defaults and raise PolypolishError with the reference's error text.
 """
+import contextlib
 import ctypes as C
 import os
 
@@ -277,6 +278,19 @@ class Packed:
             pass
 
 
+@contextlib.contextmanager
+def _report_files(ctx, changes, status, vcf, depth_bedgraph):
+    """The file-level calls on ctx inside the block also write these reports (None: off); the files are always cleared after it."""
+    setters = (ctx.set_changes_file, ctx.set_status_file, ctx.set_vcf_file, ctx.set_depth_file)
+    for set_file, path in zip(setters, (changes, status, vcf, depth_bedgraph)):
+        set_file(path)
+    try:
+        yield
+    finally:
+        for set_file in setters:
+            set_file(None)
+
+
 def pack_sams(fasta, sams, careful=False):
     p = Packed(fasta, careful)
     for s in sams:
@@ -388,12 +402,11 @@ class Context:
         prm = _params(**opts)
         cap = self._G + (1 << 20) if fetch else 0
         L = lib()
-        if changes:
-            L.pp_polish_set_changes(self.h, 1)
-        if status:
-            L.pp_polish_set_status(self.h, 1)
-        if depth_runs:
-            L.pp_polish_set_depth(self.h, 1)
+        recorders = [(set_on, get, key) for on, set_on, get, key in ((changes, L.pp_polish_set_changes, self.changes_rows, "changes"),
+                                                                     (status, L.pp_polish_set_status, self.status_runs, "status"),
+                                                                     (depth_runs, L.pp_polish_set_depth, self.depth_runs, "depth")) if on]
+        for set_on, _, _ in recorders:
+            set_on(self.h, 1)
         ok = False
         try:
             for _ in range(2):
@@ -410,55 +423,39 @@ class Context:
                 raise self._err(rc)
             ok = True
         finally:
-            if changes:
-                L.pp_polish_set_changes(self.h, 2 if ok else 0)     # a failed call leaves nothing recording
-            if status:
-                L.pp_polish_set_status(self.h, 2 if ok else 0)
-            if depth_runs:
-                L.pp_polish_set_depth(self.h, 2 if ok else 0)
+            for set_on, _, _ in recorders:
+                set_on(self.h, 2 if ok else 0)                      # a failed call leaves nothing recording
         out = self._finish(res, keep, self._nc) if fetch else dict(n_aln_used=res.n_aln_used, out_len=res.out_len, timing=res.timing.as_dict())
-        if changes:
-            out["changes"] = self.changes_rows()
-        if status:
-            out["status"] = self.status_runs()
-        if depth_runs:
-            out["depth"] = self.depth_runs()
+        for _, get, key in recorders:
+            out[key] = get()
         return out
+
+    def _runs(self, fetch, value_dtype, value_key):
+        """The runs of a per-position report (fetch = pp_polish_status_fetch / pp_polish_depth_fetch), in position order: numpy arrays
+        "start" and "end" (global positions, half-open) and the runs' values under value_key."""
+        n = C.c_uint64()
+        rc = fetch(self.h, 0, None, None, C.byref(n))
+        if rc != PP_OK:
+            raise self._err(rc)
+        start, value = np.zeros(max(1, n.value), np.uint64), np.zeros(max(1, n.value), value_dtype)
+        if n.value:
+            rc = fetch(self.h, n.value, start.ctypes.data, value.ctypes.data, C.byref(n))
+            if rc != PP_OK:
+                raise self._err(rc)
+        start, value = start[:n.value], value[:n.value]
+        end = np.append(start[1:], np.uint64(self._G)).astype(np.uint64)
+        return {"start": start, "end": end, value_key: value}
 
     def status_runs(self):
         """The status runs of the last polish with status recorded (pp_polish_status_fetch), in position order: numpy arrays
         "start" and "end" (global positions, half-open) and "status" (0 low_depth, 1 none, 2 multiple, 3 too_close, 4 kept,
         5 changed)."""
-        L = lib()
-        n = C.c_uint64()
-        rc = L.pp_polish_status_fetch(self.h, 0, None, None, C.byref(n))
-        if rc != PP_OK:
-            raise self._err(rc)
-        start, status = np.zeros(max(1, n.value), np.uint64), np.zeros(max(1, n.value), np.uint8)
-        if n.value:
-            rc = L.pp_polish_status_fetch(self.h, n.value, start.ctypes.data, status.ctypes.data, C.byref(n))
-            if rc != PP_OK:
-                raise self._err(rc)
-        start, status = start[:n.value], status[:n.value]
-        end = np.append(start[1:], np.uint64(self._G)).astype(np.uint64)
-        return dict(start=start, end=end, status=status)
+        return self._runs(lib().pp_polish_status_fetch, np.uint8, "status")
 
     def depth_runs(self):
         """The depth runs of the last polish with depth recorded (pp_polish_depth_fetch), in position order: numpy arrays "start" and
         "end" (global positions, half-open) and "tenths" (the --debug depth text times ten: 12.3 -> 123)."""
-        L = lib()
-        n = C.c_uint64()
-        rc = L.pp_polish_depth_fetch(self.h, 0, None, None, C.byref(n))
-        if rc != PP_OK:
-            raise self._err(rc)
-        start, tenths = np.zeros(max(1, n.value), np.uint64), np.zeros(max(1, n.value), np.uint64)
-        if n.value:
-            rc = L.pp_polish_depth_fetch(self.h, n.value, start.ctypes.data, tenths.ctypes.data, C.byref(n))
-            if rc != PP_OK:
-                raise self._err(rc)
-        start, tenths = start[:n.value], tenths[:n.value]
-        end = np.append(start[1:], np.uint64(self._G)).astype(np.uint64)
-        return dict(start=start, end=end, tenths=tenths)
+        return self._runs(lib().pp_polish_depth_fetch, np.uint64, "tenths")
 
     def changes_rows(self):
         """The change report of the last polish with changes recorded (pp_polish_changes_fetch), in position order: one dict per
@@ -586,18 +583,9 @@ class Context:
         arr = (C.c_char_p * max(1, len(sams)))(*[str(s).encode() for s in sams])
         out = C.c_void_p()
         n = C.c_uint64()
-        self.set_changes_file(changes)
-        self.set_status_file(status)
-        self.set_vcf_file(vcf)
-        self.set_depth_file(depth_bedgraph)
-        try:
+        with _report_files(self, changes, status, vcf, depth_bedgraph):
             rc = lib().pp_polish_files(self.h, str(assembly).encode(), arr, len(sams), C.byref(prm),
                                        str(debug).encode() if debug else None, C.byref(out), C.byref(n), int(verbose))
-        finally:
-            self.set_changes_file(None)
-            self.set_status_file(None)
-            self.set_vcf_file(None)
-            self.set_depth_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
@@ -612,19 +600,10 @@ class Context:
                                                                               C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.c_int]
         prm = _params(**opts)
         out, n = C.c_void_p(), C.c_uint64()
-        self.set_changes_file(changes)
-        self.set_status_file(status)
-        self.set_vcf_file(vcf)
-        self.set_depth_file(depth_bedgraph)
-        try:
+        with _report_files(self, changes, status, vcf, depth_bedgraph):
             rc = L.pp_filter_polish_files(self.h, str(assembly).encode(), str(in1).encode(), str(in2).encode(),
                                           str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
                                           low, high, C.byref(prm), C.byref(out), C.byref(n), int(verbose))
-        finally:
-            self.set_changes_file(None)
-            self.set_status_file(None)
-            self.set_vcf_file(None)
-            self.set_depth_file(None)
         if rc != PP_OK:
             raise self._err(rc)
         data = C.string_at(out, n.value)
@@ -884,18 +863,9 @@ def polish_files_multi(assembly, sams, devices=None, verbose=False, parser=0, co
         prm = _params(**opts)
         arr = (C.c_char_p * max(1, len(sams)))(*[str(s).encode() for s in sams])
         out, n = C.c_void_p(), C.c_uint64()
-        ctxs[0].set_changes_file(changes)
-        ctxs[0].set_status_file(status)
-        ctxs[0].set_vcf_file(vcf)
-        ctxs[0].set_depth_file(depth_bedgraph)
-        try:
+        with _report_files(ctxs[0], changes, status, vcf, depth_bedgraph):
             rc = L.pp_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), arr, len(sams), C.byref(prm), None,
                                          C.byref(out), C.byref(n), int(verbose))
-        finally:
-            ctxs[0].set_changes_file(None)
-            ctxs[0].set_status_file(None)
-            ctxs[0].set_vcf_file(None)
-            ctxs[0].set_depth_file(None)
         if rc != PP_OK:
             raise ctxs[0]._err(rc)
         data = C.string_at(out, n.value)
@@ -945,19 +915,10 @@ def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientat
 
     def run(ctxs, arr_ctx):
         out, n = C.c_void_p(), C.c_uint64()
-        ctxs[0].set_changes_file(changes)
-        ctxs[0].set_status_file(status)
-        ctxs[0].set_vcf_file(vcf)
-        ctxs[0].set_depth_file(depth_bedgraph)
-        try:
+        with _report_files(ctxs[0], changes, status, vcf, depth_bedgraph):
             rc = L.pp_filter_polish_files_multi(arr_ctx, len(ctxs), str(assembly).encode(), str(in1).encode(), str(in2).encode(),
                                                 str(out1).encode() if out1 else None, str(out2).encode() if out2 else None, orientation.encode(),
                                                 low, high, C.byref(prm), C.byref(out), C.byref(n), int(verbose))
-        finally:
-            ctxs[0].set_changes_file(None)
-            ctxs[0].set_status_file(None)
-            ctxs[0].set_vcf_file(None)
-            ctxs[0].set_depth_file(None)
         if rc != PP_OK:
             raise ctxs[0]._err(rc)
         data = C.string_at(out, n.value)

@@ -42,40 +42,6 @@ std::string qscore_text(double identity) {
 
 extern "C" void pp_free(void* p) { free(p); }
 
-// write_debug_header / write_debug_line (polish.rs:247-266): every position of the assembly, one chunk at a time; the allele strings
-// of the positions that have other alleles come from the device (k_allele_strings)
-static int write_debug_tsv(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs* contigs, FILE* f) {
-    if (fputs(pp::DEBUG_HEADER, f) < 0) return PP_ERR_IO;
-    const uint64_t CH = 1 << 18;
-    std::vector<pp_debug_pos> recs(CH);
-    std::vector<uint32_t> at;
-    std::vector<uint64_t> off;
-    std::vector<uint8_t> pool;
-    pp::DebugRows rows;
-    std::string buf;
-    for (uint32_t c = 0; c < contigs->n_contigs; ++c) {
-        const char* name = pp_fasta_name(fa, c);
-        for (uint64_t p0 = contigs->off[c]; p0 < contigs->off[c + 1]; p0 += CH) {
-            const uint64_t n = std::min<uint64_t>(CH, contigs->off[c + 1] - p0);
-            int rc = pp_polish_debug_fetch(ctx, p0, n, recs.data());
-            if (rc != PP_OK) return rc;
-            at.clear();
-            for (uint64_t i = 0; i < n; ++i)
-                if (recs[i].n_other || recs[i].new_node != 0xFFFFFFFFu) at.push_back((uint32_t)(p0 + i));
-            rc = pp_polish_debug_strings(ctx, at.data(), (uint32_t)at.size(), off, pool);
-            if (rc != PP_OK) return rc;
-            buf.clear();
-            size_t k = 0;
-            for (uint64_t i = 0; i < n; ++i) {
-                const uint8_t* al = (k < at.size() && at[k] == p0 + i) ? pool.data() + off[k++] : nullptr;
-                rows.add(buf, name, p0 + i - contigs->off[c], recs[i], al);
-            }
-            if (fwrite(buf.data(), 1, buf.size(), f) != buf.size()) return PP_ERR_IO;
-        }
-    }
-    return PP_OK;
-}
-
 // One shard on one GPU (run by its own host thread when there are several).
 struct ShardJob {
     pp_ctx* ctx = nullptr;
@@ -229,16 +195,16 @@ using FastaPtr = std::unique_ptr<pp_fasta, Deleter<pp_fasta_free>>;
 using PackPtr = std::unique_ptr<pp_pack, Deleter<pp_pack_free>>;
 using ShardsPtr = std::unique_ptr<pp_shards, Deleter<pp_shards_free>>;
 
-// --debug / --changes / --status-bed / --depth-bedgraph: the contexts record per-position data (Set = pp_polish_set_debug /
-// pp_polish_set_changes / pp_polish_set_status / pp_polish_set_depth) for the length of
-// the call.  They are left in mode 2 (not recording, the records of this call readable) when the call succeeded, otherwise in mode
-// 0, so that later calls neither record nor read stale data.
-template <int (*Set)(pp_ctx*, int)>
+// --debug / --changes / --status-bed / --depth-bedgraph: the contexts record per-position data (through pp_polish_set_debug /
+// pp_polish_set_changes / pp_polish_set_status / pp_polish_set_depth) for the length of the call.  They are left in mode 2 (not
+// recording, the records of this call readable) when the call succeeded, otherwise in mode 0, so that later calls neither record nor
+// read stale data.
 struct Recording {
-    std::vector<pp_ctx*> ctxs;
+    using Set = int (*)(pp_ctx*, int);
+    std::vector<std::pair<Set, pp_ctx*>> on;
     bool ok = false;
-    Recording(pp_ctx* const* c, int n, bool on) { if (on) for (int i = 0; i < n; ++i) { ctxs.push_back(c[i]); Set(c[i], 1); } }
-    ~Recording() { for (pp_ctx* c : ctxs) Set(c, ok ? 2 : 0); }
+    void record(Set set, pp_ctx* const* c, int n) { for (int i = 0; i < n; ++i) { on.push_back({set, c[i]}); set(c[i], 1); } }
+    ~Recording() { for (auto& [set, c] : on) set(c, ok ? 2 : 0); }
 };
 
 // What one way of loading the alignments leaves for the polish: one job per GPU, whatever backs their arrays, and what to print.
@@ -587,8 +553,44 @@ static int fetch_changes(pp_ctx* ctx, const std::vector<ShardJob>& jobs, ChangeR
     return PP_OK;
 }
 
+// write_debug_header / write_debug_line (polish.rs:247-266): every position of the assembly, one chunk at a time; the allele strings
+// of the positions that have other alleles come from the device (k_allele_strings).  PP_ERR_CUDA: its message is on ctx; any other
+// error is PP_ERR_IO, the file could not be written.
+static int write_debug_tsv(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>&, const ChangeRows&,
+                           FILE* f) {
+    if (fputs(pp::DEBUG_HEADER, f) < 0) return PP_ERR_IO;
+    const uint64_t CH = 1 << 18;
+    std::vector<pp_debug_pos> recs(CH);
+    std::vector<uint32_t> at;
+    std::vector<uint64_t> off;
+    std::vector<uint8_t> pool;
+    pp::DebugRows rows;
+    std::string buf;
+    for (uint32_t c = 0; c < contigs.n_contigs; ++c) {
+        const char* name = pp_fasta_name(fa, c);
+        for (uint64_t p0 = contigs.off[c]; p0 < contigs.off[c + 1]; p0 += CH) {
+            const uint64_t n = std::min<uint64_t>(CH, contigs.off[c + 1] - p0);
+            int rc = pp_polish_debug_fetch(ctx, p0, n, recs.data());
+            if (rc != PP_OK) return rc == PP_ERR_CUDA ? rc : PP_ERR_IO;
+            at.clear();
+            for (uint64_t i = 0; i < n; ++i)
+                if (recs[i].n_other || recs[i].new_node != 0xFFFFFFFFu) at.push_back((uint32_t)(p0 + i));
+            rc = pp_polish_debug_strings(ctx, at.data(), (uint32_t)at.size(), off, pool);
+            if (rc != PP_OK) return rc == PP_ERR_CUDA ? rc : PP_ERR_IO;
+            buf.clear();
+            size_t k = 0;
+            for (uint64_t i = 0; i < n; ++i) {
+                const uint8_t* al = (k < at.size() && at[k] == p0 + i) ? pool.data() + off[k++] : nullptr;
+                rows.add(buf, name, p0 + i - contigs.off[c], recs[i], al);
+            }
+            if (fwrite(buf.data(), 1, buf.size(), f) != buf.size()) return PP_ERR_IO;
+        }
+    }
+    return PP_OK;
+}
+
 // --changes: the --debug header, then the --debug rows of the changed positions.  PP_ERR_IO: the file could not be written.
-static int write_changes(const pp_fasta* fa, const ChangeRows& cr, FILE* f) {
+static int write_changes(pp_ctx*, const pp_fasta* fa, const pp_contigs&, const std::vector<ShardJob>&, const ChangeRows& cr, FILE* f) {
     std::string buf = pp::DEBUG_HEADER;
     pp::DebugRows rows;
     for (const ChangeRows::Row& r : cr.order) rows.add(buf, pp_fasta_name(fa, r.contig), r.pos, cr.rec(r), cr.alleles(r));
@@ -614,7 +616,7 @@ static bool emitted_allele(const pp_debug_pos& r, const uint8_t* al, std::string
 
 // --vcf: the header, then per contig in the input FASTA's order the records vcf_records.h makes of its draft and its change rows.
 // PP_ERR_IO: the file could not be written; another error: its message is on ctx.
-static int write_vcf(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const ChangeRows& cr, FILE* f) {
+static int write_vcf(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>&, const ChangeRows& cr, FILE* f) {
     std::string buf;
     pp::vcf_header_begin(buf);
     for (uint32_t c = 0; c < contigs.n_contigs; ++c) pp::vcf_header_contig(buf, pp_fasta_name(fa, c), contigs.off[c + 1] - contigs.off[c]);
@@ -641,7 +643,7 @@ static int write_vcf(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs,
 // of its own contigs; a run never crosses a contig, so each contig's lines are its runs in order.  PP_ERR_IO: the file could not be
 // written; another error: its message is on ctx.
 template <class T, int (*Fetch)(pp_ctx*, uint64_t, uint64_t*, T*, uint64_t*), void (*Text)(std::string&, T)>
-static int write_runs(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>& jobs, FILE* f) {
+static int write_runs(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>& jobs, const ChangeRows&, FILE* f) {
     struct Run { uint64_t start, end; T value; };
     std::vector<std::vector<Run>> by_contig(contigs.n_contigs);
     for (const ShardJob& j : jobs) {
@@ -678,6 +680,14 @@ static void status_text(std::string& buf, uint8_t status) {
 static constexpr auto write_status_bed = write_runs<uint8_t, pp_polish_status_fetch, status_text>;
 static constexpr auto write_depth_bedgraph = write_runs<uint64_t, pp_polish_depth_fetch, pp::depth_text>;
 
+// One report file of polish_files_impl: its path ("" = not asked for), the open file and what writes it.
+struct ReportFile {
+    std::string path;
+    int (*write)(pp_ctx*, const pp_fasta*, const pp_contigs&, const std::vector<ShardJob>&, const ChangeRows&, FILE*);
+    FILE* f = nullptr;
+    ~ReportFile() { if (f) fclose(f); }
+};
+
 static void print_timing(const Load& ld) {
     fputs(ld.timing.c_str(), stderr);
     for (uint32_t s = 0; s < ld.jobs.size(); ++s) {
@@ -706,28 +716,19 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     if (!pp::file_exists(assembly)) return pp_ctx_fail(ctx, PP_ERR_INPUT, ("\"" + std::string(assembly) + "\" file does not exist").c_str());
     for (int i = 0; i < n_sams; ++i)
         if (!pp::file_exists(sams[i])) return pp_ctx_fail(ctx, PP_ERR_INPUT, ("\"" + std::string(sams[i]) + "\" file does not exist").c_str());
-    const bool debug = debug_path && debug_path[0];
-    const std::string changes_path = pp_ctx_changes_file(ctx), status_path = pp_ctx_status_file(ctx), vcf_path = pp_ctx_vcf_file(ctx),
-                      depth_path = pp_ctx_depth_file(ctx);
-    const bool changes = !changes_path.empty(), status = !status_path.empty(), vcf = !vcf_path.empty(), depth = !depth_path.empty();
-    FILE *debug_file = nullptr, *changes_file = nullptr, *status_file = nullptr, *vcf_file = nullptr, *depth_file = nullptr;
-    struct FileCloser { FILE*& f; ~FileCloser() { if (f) fclose(f); } } closer{debug_file}, closer2{changes_file}, closer3{status_file},
-        closer4{vcf_file}, closer5{depth_file};
+    // the reports in the order they are created and written: --debug, then the per-context report files
+    ReportFile reports[] = {{debug_path ? debug_path : "", write_debug_tsv}, {ctx->report_path[F_CHANGES], write_changes},
+                            {ctx->report_path[F_STATUS], write_status_bed}, {ctx->report_path[F_VCF], write_vcf},
+                            {ctx->report_path[F_DEPTH], write_depth_bedgraph}};
+    const bool debug = !reports[0].path.empty(), changes = !reports[1 + F_CHANGES].path.empty(), vcf = !reports[1 + F_VCF].path.empty();
     // create_debug_file polish.rs:230-244; the other reports are worded like it
-    auto create = [ctx](const std::string& path, FILE*& file) {
-        file = fopen(path.c_str(), "wb");
-        return file ? PP_OK : pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + path + "\"").c_str());
-    };
-    int created = debug ? create(debug_path, debug_file) : PP_OK;
-    if (created == PP_OK && changes) created = create(changes_path, changes_file);
-    if (created == PP_OK && status) created = create(status_path, status_file);
-    if (created == PP_OK && vcf) created = create(vcf_path, vcf_file);
-    if (created == PP_OK && depth) created = create(depth_path, depth_file);
-    if (created != PP_OK) return created;
-    Recording<pp_polish_set_debug> recording(&ctx, 1, debug);
-    Recording<pp_polish_set_changes> recording_changes(ctxs, n_ctx, changes || vcf);
-    Recording<pp_polish_set_status> recording_status(ctxs, n_ctx, status);
-    Recording<pp_polish_set_depth> recording_depth(ctxs, n_ctx, depth);
+    for (ReportFile& r : reports)
+        if (!r.path.empty() && !(r.f = fopen(r.path.c_str(), "wb"))) return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to create \"" + r.path + "\"").c_str());
+    Recording recording;
+    if (debug) recording.record(pp_polish_set_debug, &ctx, 1);
+    if (changes || vcf) recording.record(pp_polish_set_changes, ctxs, n_ctx);
+    if (reports[1 + F_STATUS].f) recording.record(pp_polish_set_status, ctxs, n_ctx);
+    if (reports[1 + F_DEPTH].f) recording.record(pp_polish_set_depth, ctxs, n_ctx);
 
     // the first SAM file starts streaming into HBM while the assembly is loaded
     const bool device_parser = pp_get_parser(ctx) == 0;
@@ -772,30 +773,17 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
         }
     }
     if (rc == PP_OK) rc = job_error(ctx, ld);
-    if (rc == PP_OK && debug) {
-        rc = write_debug_tsv(ctx, fa.get(), &contigs, debug_file);
-        if (rc != PP_OK && rc != PP_ERR_CUDA) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + std::string(debug_path) + "\"").c_str());
-    }
     ChangeRows change_rows;
-    if (rc == PP_OK && (changes || vcf)) rc = fetch_changes(ctx, ld.jobs, change_rows);
-    if (rc == PP_OK && changes) {
-        rc = write_changes(fa.get(), change_rows, changes_file);
-        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + changes_path + "\"").c_str());
-    }
-    if (rc == PP_OK && status) {
-        rc = write_status_bed(ctx, fa.get(), contigs, ld.jobs, status_file);
-        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + status_path + "\"").c_str());
-    }
-    if (rc == PP_OK && vcf) {
-        rc = write_vcf(ctx, fa.get(), contigs, change_rows, vcf_file);
-        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + vcf_path + "\"").c_str());
-    }
-    if (rc == PP_OK && depth) {
-        rc = write_depth_bedgraph(ctx, fa.get(), contigs, ld.jobs, depth_file);
-        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + depth_path + "\"").c_str());
+    for (size_t i = 0; rc == PP_OK && i < std::size(reports); ++i) {
+        // the change rows once, after the debug TSV: both make their allele strings in the same device pool, and the change rows'
+        // strings stay there for pp_polish_changes_fetch
+        if (i == 1 + F_CHANGES && (changes || vcf)) rc = fetch_changes(ctx, ld.jobs, change_rows);
+        if (rc != PP_OK || !reports[i].f) continue;
+        rc = reports[i].write(ctx, fa.get(), contigs, ld.jobs, change_rows, reports[i].f);
+        if (rc == PP_ERR_IO) rc = pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write to file \"" + reports[i].path + "\"").c_str());
     }
     if (rc != PP_OK) return rc;
-    recording.ok = recording_changes.ok = recording_status.ok = recording_depth.ok = true;
+    recording.ok = true;
     if (verbose) {
         uint64_t n_used = 0;
         for (const ShardJob& j : ld.jobs) n_used += j.res.n_aln_used;
@@ -865,12 +853,15 @@ extern "C" int pp_filter_polish_files_multi(pp_ctx* const* ctxs, int n_ctx, cons
     return pp_filter_polish_files(ctx, assembly, in1, in2, out1, out2, orientation, low, high, prm, out_fasta, out_len, verbose);
 }
 
-extern "C" int pp_set_vcf_file(pp_ctx* ctx, const char* path) {
+static int set_report_file(pp_ctx* ctx, int which, const char* path) {
     if (!ctx) return PP_ERR_ARG;
-    ctx->vcf_path = path ? path : "";
+    ctx->report_path[which] = path ? path : "";
     return PP_OK;
 }
-const char* pp_ctx_vcf_file(pp_ctx* ctx) { return ctx->vcf_path.c_str(); }
+extern "C" int pp_set_changes_file(pp_ctx* ctx, const char* path) { return set_report_file(ctx, F_CHANGES, path); }
+extern "C" int pp_set_status_file(pp_ctx* ctx, const char* path) { return set_report_file(ctx, F_STATUS, path); }
+extern "C" int pp_set_vcf_file(pp_ctx* ctx, const char* path) { return set_report_file(ctx, F_VCF, path); }
+extern "C" int pp_set_depth_file(pp_ctx* ctx, const char* path) { return set_report_file(ctx, F_DEPTH, path); }
 
 extern "C" int pp_polish_files(pp_ctx* ctx, const char* assembly, const char* const* sams, int n_sams,
                                const pp_polish_params* prm, const char* debug_path, char** out_fasta,

@@ -380,9 +380,9 @@ static const char* err_text(unsigned code) {
 // depth keys are padded the same way (depth_key_bytes)
 static size_t status_bytes(uint64_t G) { return (size_t)((G + SR_CHUNK - 1) / SR_CHUNK) * SR_CHUNK + 16; }
 
-// A call's status bytes or depth keys -> its runs in b[b_start] / b[b_value], sized from the count (*n_runs).
+// A call's status bytes or depth keys -> the runs of report r, sized from their count.
 template <class T>
-static int report_runs(pp_ctx* ctx, const T* e, int b_start, int b_value, uint32_t* n_runs) {
+static int report_runs(pp_ctx* ctx, const T* e, RunReport& r) {
     cudaStream_t s = ctx->stream;
     const uint32_t G = (uint32_t)ctx->G, n_blk = (uint32_t)((ctx->G + SR_CHUNK - 1) / SR_CHUNK);
     CK(ctx->b[B_RUNFIRST].ensure(((size_t)n_blk + 1) * 4));
@@ -398,11 +398,12 @@ static int report_runs(pp_ctx* ctx, const T* e, int b_start, int b_value, uint32
     CK(cudaMemcpyAsync(&n, first + n_blk, 4, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     CK(cudaGetLastError());
-    CK(ctx->b[b_start].ensure((size_t)n * 4 + 4)); CK(ctx->b[b_value].ensure((size_t)n * sizeof(T) + 8));
-    if (n_blk) k_status_runs<T><<<n_blk, SR_THREADS, 0, s>>>(e, G, first, ctx->b[b_start].as<uint32_t>(), ctx->b[b_value].as<T>());
+    CK(ctx->b[r.b_start].ensure((size_t)n * 4 + 4)); CK(ctx->b[r.b_value].ensure((size_t)n * sizeof(T) + 8));
+    if (n_blk) k_status_runs<T><<<n_blk, SR_THREADS, 0, s>>>(e, G, first, ctx->b[r.b_start].as<uint32_t>(), ctx->b[r.b_value].as<T>());
     CK(cudaGetLastError());
     ctx->launches += 2;
-    *n_runs = n;
+    r.n = n;
+    r.have = true;
     return PP_OK;
 }
 
@@ -421,7 +422,7 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
     const uint64_t G = ctx->G, n_aln = ctx->n_aln;
     const uint32_t n_tiles = (uint32_t)((G + TL_T - 1) / TL_T);              // = vote / compaction chunks
     const size_t padG = (size_t)n_tiles * TL_T + 16;                          // k_tile / k_compact move whole chunks with vector accesses
-    ctx->have_changes = ctx->have_status = ctx->have_depth = false;
+    ctx->have_changes = ctx->status.have = ctx->depth.have = false;
 
     CK(ctx->b[B_OUTOFF].ensure(((size_t)ctx->n_contigs + 1) * 8));
     CK(ctx->b[B_RES].ensure(padG * 2)); CK(ctx->b[B_RECAT].ensure((G + 1) * 4)); CK(ctx->b[B_CHUNKDELTA].ensure((size_t)n_tiles * 8));
@@ -456,8 +457,8 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
         CK(ctx->b[B_OUT].ensure(out_cap + 64));
         // --depth-bedgraph / --status-bed: the depth keys, then the status bytes, in one buffer (VoteParams::sts), allocated before the
         // timed stages
-        const size_t key_bytes = ctx->depth_on ? depth_key_bytes(G) : 0;
-        if (ctx->status_on || ctx->depth_on) CK(ctx->b[B_STS].ensure(key_bytes + (ctx->status_on ? status_bytes(G) : 16)));
+        const size_t key_bytes = ctx->depth.on ? depth_key_bytes(G) : 0;
+        if (ctx->status.on || ctx->depth.on) CK(ctx->b[B_STS].ensure(key_bytes + (ctx->status.on ? status_bytes(G) : 16)));
 
         DevData d;
         fill_data(ctx, d);
@@ -510,9 +511,9 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
             CK(ctx->b[B_CHG].ensure((size_t)ctx->chg_cap * sizeof(pp_debug_pos))); CK(ctx->b[B_CHGPOS].ensure((size_t)ctx->chg_cap * 4));
             vp.chg = ctx->b[B_CHG].as<pp_debug_pos>(); vp.chg_pos = ctx->b[B_CHGPOS].as<uint32_t>(); vp.chg_cap = ctx->chg_cap;
         }
-        vp.sts = (ctx->status_on || ctx->depth_on) ? ctx->b[B_STS].as<uint8_t>() : nullptr;
+        vp.sts = (ctx->status.on || ctx->depth.on) ? ctx->b[B_STS].as<uint8_t>() : nullptr;
         {
-            const TileKernel kt = tile_kernel<BITS>(vp.chg, ctx->status_on, ctx->depth_on);
+            const TileKernel kt = tile_kernel<BITS>(vp.chg, ctx->status.on, ctx->depth.on);
             int occ = 1;
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kt, TL_THREADS, sizeof(TileShared)));
             const uint32_t grid = std::min<uint32_t>(n_tiles, (uint32_t)ctx->sm_count * (uint32_t)std::max(occ, 1));   // persistent: tiles by ticket
@@ -557,15 +558,13 @@ static int run_polish(pp_ctx* ctx, const pp_polish_params* prm, pp_polish_result
 
         ctx->have_debug = ctx->debug_on; ctx->last_head = d.oth_head; ctx->last_nodes = std::min(hs.node_count, node_cap);
         ctx->have_changes = ctx->changes_on; ctx->n_changes = ctx->changes_on ? hs.n_changes : 0; ctx->chg_pool = -1;
-        if (ctx->status_on) {
-            const int rc = report_runs(ctx, vp.sts + key_bytes, B_RUNSTART, B_RUNSTS, &ctx->n_runs);
+        if (ctx->status.on) {
+            const int rc = report_runs(ctx, vp.sts + key_bytes, ctx->status);
             if (rc != PP_OK) return rc;
-            ctx->have_status = true;
         }
-        if (ctx->depth_on) {
-            const int rc = report_runs(ctx, reinterpret_cast<const unsigned long long*>(vp.sts), B_DEPSTART, B_DEPRUN, &ctx->n_dep_runs);
+        if (ctx->depth.on) {
+            const int rc = report_runs(ctx, reinterpret_cast<const unsigned long long*>(vp.sts), ctx->depth);
             if (rc != PP_OK) return rc;
-            ctx->have_depth = true;
         }
         res->out_len = hs.out_len;
         res->n_aln_used = hs.n_used;
@@ -719,13 +718,6 @@ extern "C" int pp_polish_set_changes(pp_ctx* ctx, int on) {
     return PP_OK;
 }
 
-extern "C" int pp_set_changes_file(pp_ctx* ctx, const char* path) {
-    if (!ctx) return PP_ERR_ARG;
-    ctx->changes_path = path ? path : "";
-    return PP_OK;
-}
-const char* pp_ctx_changes_file(pp_ctx* ctx) { return ctx->changes_path.c_str(); }
-
 extern "C" int pp_polish_changes_fetch(pp_ctx* ctx, uint64_t row_cap, uint64_t* pos, pp_debug_pos* rows, uint64_t* pool_off, uint8_t* pool,
                                        uint64_t pool_cap, uint64_t* n_rows, uint64_t* pool_bytes) {
     if (!ctx) return PP_ERR_ARG;
@@ -762,70 +754,44 @@ extern "C" int pp_polish_changes_fetch(pp_ctx* ctx, uint64_t row_cap, uint64_t* 
     return PP_OK;
 }
 
-extern "C" int pp_polish_set_status(pp_ctx* ctx, int on) {
-    if (!ctx) return PP_ERR_ARG;
-    ctx->status_on = on == 1;           // 2 = stop recording but keep the last call's runs readable
+// pp_polish_set_status / pp_polish_set_depth: on = 1 records report r from the next call on; 2 stops recording but keeps the last
+// call's runs readable; 0 forgets them.
+static int set_runs(pp_ctx* ctx, RunReport& r, int on) {
+    r.on = on == 1;
     if (on != 1) { CK(cudaSetDevice(ctx->device)); ctx->b[B_STS].release(); ctx->b[B_RUNFIRST].release(); }
-    if (on == 0) { ctx->have_status = false; ctx->b[B_RUNSTART].release(); ctx->b[B_RUNSTS].release(); }
+    if (on == 0) { r.have = false; ctx->b[r.b_start].release(); ctx->b[r.b_value].release(); }
     return PP_OK;
 }
 
-extern "C" int pp_set_status_file(pp_ctx* ctx, const char* path) {
-    if (!ctx) return PP_ERR_ARG;
-    ctx->status_path = path ? path : "";
+// pp_polish_status_fetch / pp_polish_depth_fetch: the runs of report r, which the messages name `what` ("status" / "depth").
+template <class T>
+static int fetch_runs(pp_ctx* ctx, const RunReport& r, const char* what, uint64_t run_cap, uint64_t* start, T* value, uint64_t* n_runs) {
+    const std::string fn = std::string("pp_polish_") + what + "_fetch";
+    if (!r.have) return ctx->fail(PP_ERR_ARG, fn + ": the last polish did not record " + what + " (pp_polish_set_" + what + ")");
+    if (!n_runs) return ctx->fail(PP_ERR_ARG, fn + ": null size pointer");
+    const uint32_t n = r.n;
+    *n_runs = n;
+    if (run_cap == 0 && n > 0) return PP_OK;                                                   // size query
+    if (run_cap < n || (n && (!start || !value))) return ctx->fail(PP_ERR_ARG, fn + ": buffers too small");
+    CK(cudaSetDevice(ctx->device));
+    std::vector<uint32_t> st(n);
+    if (n) {
+        CK(cudaMemcpyAsync(st.data(), ctx->b[r.b_start].p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(value, ctx->b[r.b_value].p, (size_t)n * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::copy(st.begin(), st.end(), start);
     return PP_OK;
 }
-const char* pp_ctx_status_file(pp_ctx* ctx) { return ctx->status_path.c_str(); }
+
+extern "C" int pp_polish_set_status(pp_ctx* ctx, int on) { return ctx ? set_runs(ctx, ctx->status, on) : PP_ERR_ARG; }
 
 extern "C" int pp_polish_status_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint8_t* status, uint64_t* n_runs) {
-    if (!ctx) return PP_ERR_ARG;
-    if (!ctx->have_status) return ctx->fail(PP_ERR_ARG, "pp_polish_status_fetch: the last polish did not record status (pp_polish_set_status)");
-    if (!n_runs) return ctx->fail(PP_ERR_ARG, "pp_polish_status_fetch: null size pointer");
-    const uint32_t n = ctx->n_runs;
-    *n_runs = n;
-    if (run_cap == 0 && n > 0) return PP_OK;                                                   // size query
-    if (run_cap < n || (n && (!start || !status))) return ctx->fail(PP_ERR_ARG, "pp_polish_status_fetch: buffers too small");
-    CK(cudaSetDevice(ctx->device));
-    std::vector<uint32_t> st(n);
-    if (n) {
-        CK(cudaMemcpyAsync(st.data(), ctx->b[B_RUNSTART].p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(status, ctx->b[B_RUNSTS].p, n, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    std::copy(st.begin(), st.end(), start);
-    return PP_OK;
+    return ctx ? fetch_runs(ctx, ctx->status, "status", run_cap, start, status, n_runs) : PP_ERR_ARG;
 }
 
-extern "C" int pp_polish_set_depth(pp_ctx* ctx, int on) {
-    if (!ctx) return PP_ERR_ARG;
-    ctx->depth_on = on == 1;            // 2 = stop recording but keep the last call's runs readable
-    if (on != 1) { CK(cudaSetDevice(ctx->device)); ctx->b[B_STS].release(); ctx->b[B_RUNFIRST].release(); }
-    if (on == 0) { ctx->have_depth = false; ctx->b[B_DEPSTART].release(); ctx->b[B_DEPRUN].release(); }
-    return PP_OK;
-}
-
-extern "C" int pp_set_depth_file(pp_ctx* ctx, const char* path) {
-    if (!ctx) return PP_ERR_ARG;
-    ctx->depth_path = path ? path : "";
-    return PP_OK;
-}
-const char* pp_ctx_depth_file(pp_ctx* ctx) { return ctx->depth_path.c_str(); }
+extern "C" int pp_polish_set_depth(pp_ctx* ctx, int on) { return ctx ? set_runs(ctx, ctx->depth, on) : PP_ERR_ARG; }
 
 extern "C" int pp_polish_depth_fetch(pp_ctx* ctx, uint64_t run_cap, uint64_t* start, uint64_t* tenths, uint64_t* n_runs) {
-    if (!ctx) return PP_ERR_ARG;
-    if (!ctx->have_depth) return ctx->fail(PP_ERR_ARG, "pp_polish_depth_fetch: the last polish did not record depth (pp_polish_set_depth)");
-    if (!n_runs) return ctx->fail(PP_ERR_ARG, "pp_polish_depth_fetch: null size pointer");
-    const uint32_t n = ctx->n_dep_runs;
-    *n_runs = n;
-    if (run_cap == 0 && n > 0) return PP_OK;                                                   // size query
-    if (run_cap < n || (n && (!start || !tenths))) return ctx->fail(PP_ERR_ARG, "pp_polish_depth_fetch: buffers too small");
-    CK(cudaSetDevice(ctx->device));
-    std::vector<uint32_t> st(n);
-    if (n) {
-        CK(cudaMemcpyAsync(st.data(), ctx->b[B_DEPSTART].p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaMemcpyAsync(tenths, ctx->b[B_DEPRUN].p, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    std::copy(st.begin(), st.end(), start);
-    return PP_OK;
+    return ctx ? fetch_runs(ctx, ctx->depth, "depth", run_cap, start, tenths, n_runs) : PP_ERR_ARG;
 }

@@ -35,6 +35,18 @@ enum { B_CONTIG, B_REFSTART, B_READID, B_SEQOFF, B_SEQLEN, B_CIGOFF, B_NCIG, B_N
        B_DEPSTART, B_DEPRUN,
        B_TOKLINE, B_TOKTMP, B_TOKNAMES, B_COUNT };
 
+// A per-position report recorded as runs: whether calls record it (on), whether the last call did (have) and its runs, exactly n
+// long, in b[b_start] (start positions) / b[b_value] (values).
+struct RunReport {
+    bool on, have;
+    uint32_t n;
+    int b_start, b_value;
+};
+
+// The report files of the file-level commands that are set per context (pp_set_changes_file, pp_set_status_file, pp_set_vcf_file,
+// pp_set_depth_file), in the order they are created after --debug's.
+enum { F_CHANGES, F_STATUS, F_VCF, F_DEPTH, F_COUNT };
+
 struct pp_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -65,16 +77,9 @@ struct pp_ctx {
     bool changes_on = false, have_changes = false;
     uint32_t chg_cap = 0, n_changes = 0;
     int64_t chg_pool = -1;                // bytes of the change rows' allele strings in B_STRPOOL, -1 = not made yet
-    std::string changes_path;             // pp_set_changes_file: the report the file-level commands also write
-    // --status-bed (pp_polish_set_status): the status runs of the last call (B_RUNSTART / B_RUNSTS, exactly n_runs long)
-    bool status_on = false, have_status = false;
-    uint32_t n_runs = 0;
-    std::string status_path;              // pp_set_status_file: the BED the file-level commands also write
-    // --depth-bedgraph (pp_polish_set_depth): the depth runs of the last call (B_DEPSTART / B_DEPRUN, exactly n_dep_runs long)
-    bool depth_on = false, have_depth = false;
-    uint32_t n_dep_runs = 0;
-    std::string depth_path;               // pp_set_depth_file: the bedGraph the file-level commands also write
-    std::string vcf_path;                 // pp_set_vcf_file: the VCF the file-level commands also write (from the change rows)
+    // --status-bed (pp_polish_set_status) and --depth-bedgraph (pp_polish_set_depth): each one's runs of the last call
+    RunReport status{false, false, 0, B_RUNSTART, B_RUNSTS}, depth{false, false, 0, B_DEPSTART, B_DEPRUN};
+    std::string report_path[F_COUNT];     // pp_set_*_file: the reports the file-level commands also write ("" = none)
     TokState* tok = nullptr;              // SAM tokeniser state (tok_kernels.cu), created on first use
     int parser = 0;                       // pp_set_parser: 0 device tokeniser where possible, 1 host packer only
 

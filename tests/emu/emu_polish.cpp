@@ -1,9 +1,18 @@
 // emu_polish.cpp — runs the polish kernels of polypolish_b200/csrc/polish_dev.cuh on the CPU (tests/emu/cuda_emu.h): the same
-// device code, one OS thread per CUDA thread, so that the kernels' logic is checked against the oracle without a GPU.
-// TEST INFRASTRUCTURE: built and used by tests/test_emu_polish.py only; nothing in polypolish_b200/ links or loads this.
+// device code, one OS thread per CUDA thread, so that the kernels' logic is checked against the oracle without a GPU.  On request it
+// records the per-position reports the way the product does, from the k_tile<BITS, CHG, STS, DEP> instance the product would run:
+//   changes: k_tile's change list, then k_allele_strings over it, then the product's row formatter (debug_rows.h);
+//   debug:   k_tile's record of every position (vp.dbg), k_allele_strings over the positions that have other alleles or emit a node,
+//            and the same formatter;
+//   status / depth: k_tile's status bytes / depth keys (one buffer, keys first, as in the product), then k_status_heads<T>, the
+//            exclusive scan of its counts (CUB's on the device, std::exclusive_scan here) and k_status_runs<T>, then the runs as the
+//            lines `polish --status-bed` / `polish --depth-bedgraph` write.
+// Also depth_tenths and the host's depth text against snprintf("%.1f").
+// TEST INFRASTRUCTURE: built and used by tests/emu_lib.py only; nothing in polypolish_b200/ links or loads this.
 #include "cuda_emu.h"
 
 #include "../../polypolish_b200/csrc/polish_dev.cuh"
+#include "../../polypolish_b200/csrc/debug_rows.h"
 
 #include <numeric>
 #include <string>
@@ -14,6 +23,9 @@ static std::vector<uint32_t> g_last_bin_start, g_last_sval, g_last_tile_order;
 
 namespace {
 
+// emu_polish_reports' `reports` bits, in the order of its `texts`
+enum { R_CHANGES = 1, R_DEBUG = 2, R_STATUS = 4, R_DEPTH = 8, N_REPORTS = 4 };
+
 void init_comp_table() {
     for (int i = 0; i < 256; ++i) c_comp[i] = 'N';
     const char* a = "ATGCNRYSWKMBVDH.-?";
@@ -21,9 +33,49 @@ void init_comp_table() {
     for (int i = 0; a[i]; ++i) c_comp[(unsigned char)a[i]] = (uint8_t)b[i];
 }
 
+// k_allele_strings over the records rec[i] at positions pos[i]: the pool and each record's offset in it
 template <int BITS>
+void allele_strings(const OthCtx& oc, const uint32_t* pos, const pp_debug_pos* rec, bool debug, uint32_t n, std::vector<uint8_t>& pool,
+                    std::vector<unsigned long long>& off) {
+    pool.assign(1, 0);
+    off.assign(n + 1, 0);
+    for (int attempt = 0; attempt < 2; ++attempt) {         // (the first round finds the pool's size)
+        unsigned long long used = 0;
+        emu::launch(2, 64, 0, [&] { allele_strings_body<BITS>(oc, pos, rec, debug, n, pool.data(), pool.size(), &used, off.data()); });
+        if (used <= pool.size()) break;
+        pool.resize(used);
+    }
+}
+
+// The runs of one report as "<contig>\t<start>\t<end>\t<value>" lines, the value written by text (false: a value out of range); 101:
+// the runs are malformed (a value out of range, an empty run or one that crosses a contig).
+template <class T, class Text>
+int runs_text(const pp_contigs* c, const T* e, const char* const* names, Text text, std::string* out) {
+    const uint64_t G = c->off[c->n_contigs];
+    const uint32_t n_blk = (uint32_t)((G + SR_CHUNK - 1) / SR_CHUNK);
+    std::vector<uint32_t> first(n_blk + 1, 0);
+    emu::launch(n_blk, SR_THREADS, sizeof(RunShared), [&] { status_heads_body(e, (uint32_t)G, first.data(), *(RunShared*)emu::shared_base()); });
+    std::exclusive_scan(first.begin(), first.end(), first.begin(), 0u);
+    const uint32_t n = first[n_blk];
+    std::vector<uint32_t> start(n + 1, 0xEEEEEEEEu);
+    std::vector<T> value(n + 1, (T)0xEE);
+    emu::launch(n_blk, SR_THREADS, sizeof(RunShared), [&] {
+        status_runs_body(e, (uint32_t)G, first.data(), start.data(), value.data(), *(RunShared*)emu::shared_base());
+    });
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t ctg = (uint32_t)(std::upper_bound(c->off, c->off + c->n_contigs + 1, (uint64_t)start[i]) - c->off) - 1;
+        const uint64_t end = i + 1 < n ? start[i + 1] : G;
+        if (end <= start[i] || end > c->off[ctg + 1]) return 101;
+        *out += std::string(names[ctg]) + "\t" + std::to_string(start[i] - c->off[ctg]) + "\t" + std::to_string(end - c->off[ctg]) + "\t";
+        if (!text(*out, value[i])) return 101;
+        *out += "\n";
+    }
+    return 0;
+}
+
+template <int BITS, bool CHG, bool STS, bool DEP>
 int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles, bool global_k,
-        uint64_t* err_out) {
+        bool debug, uint64_t* err_out, const char* const* names, std::string* texts) {
     const uint64_t G = c->off[c->n_contigs], n_aln = a->n_aln;
     const uint32_t n_tiles = (uint32_t)((G + TL_T - 1) / TL_T), n_bins = (uint32_t)((G + PP_BIN - 1) >> PP_BIN_SHIFT);
     const size_t padG = (size_t)n_tiles * TL_T + 16;
@@ -71,7 +123,17 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
     VoteParams vp;
     vp.n_chunks = n_tiles; vp.out = out.data(); vp.out_cap = out_cap; vp.out_off = out_off.data(); vp.changed = changed.data();
     vp.zero_depth = zero.data(); vp.total_depth = tdepth.data(); vp.res = resv.data(); vp.rec_at = rec_at.data(); vp.chunk_delta = chunk_delta.data();
-    vp.dbg = nullptr;
+    std::vector<pp_debug_pos> dbg(debug ? G + 1 : 0);
+    vp.dbg = debug ? dbg.data() : nullptr;
+    // the change list, with room for every position: it never overflows here
+    std::vector<pp_debug_pos> chg(G + 1);
+    std::vector<uint32_t> chg_pos(G + 1);
+    vp.chg = CHG ? chg.data() : nullptr; vp.chg_pos = CHG ? chg_pos.data() : nullptr; vp.chg_n = &st.n_changes; vp.chg_cap = CHG ? (uint32_t)chg.size() : 0;
+    // the depth keys, then the status bytes, padded like the product's (run_polish in polish_kernels.cu); the padding is never read
+    const uint32_t n_blk = (uint32_t)((G + SR_CHUNK - 1) / SR_CHUNK);
+    const size_t key_bytes = DEP ? depth_key_bytes(G) : 0;
+    std::vector<uint4> rep16((key_bytes + (STS ? (size_t)n_blk * SR_CHUNK + 16 : 16) + 15) / 16, make_uint4(0xA5A5A5A5u, 0xA5A5A5A5u, 0xA5A5A5A5u, 0xA5A5A5A5u));
+    vp.sts = STS || DEP ? (uint8_t*)rep16.data() : nullptr;
 
     // ---- once per dataset: bin, stable sort, bounds, permute
     if (n_aln) {
@@ -111,10 +173,60 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
             if (global_k) goodk_body<true>(d, sh); else goodk_body<false>(d, sh);
         });
     emu::launch((unsigned)std::max(1, std::min<int>(grid_tiles, (int)n_tiles)), TL_THREADS, sizeof(TileShared), [&] {
-        tile_body<BITS>(d, vp, *(TileShared*)emu::shared_base());
+        tile_body<BITS, CHG, STS, DEP>(d, vp, *(TileShared*)emu::shared_base());
     });
     emu::launch(n_tiles, VT_THREADS, sizeof(CompactShared), [&] { compact_body<BITS>(d, vp, *(CompactShared*)emu::shared_base()); });
 
+    if (st.err == ~0ull) {
+        OthCtx oc;
+        oc.nodes = d.nodes; oc.head = d.oth_head; oc.sr = SeqRef{d.seq_pool, d.seq_off, d.seq_len, d.flags};
+        std::vector<uint8_t> pool;
+        std::vector<unsigned long long> off;
+        pp::DebugRows rows;
+        if (CHG) {                                          // k_allele_strings over the list, then the rows in position order
+            const uint32_t n = st.n_changes;
+            allele_strings<BITS>(oc, chg_pos.data(), chg.data(), false, n, pool, off);
+            std::vector<uint32_t> order(n);
+            std::iota(order.begin(), order.end(), 0u);
+            std::sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return chg_pos[x] < chg_pos[y]; });
+            texts[0] = pp::DEBUG_HEADER;
+            for (uint32_t i : order) {
+                const uint32_t ctg = (uint32_t)(std::upper_bound(c->off, c->off + c->n_contigs + 1, (uint64_t)chg_pos[i]) - c->off) - 1;
+                rows.add(texts[0], names[ctg], chg_pos[i] - c->off[ctg], chg[i], pool.data() + off[i]);
+            }
+        }
+        if (debug) {                                        // every position: the strings of those with other alleles or a node
+            std::vector<uint32_t> at;
+            for (uint64_t p = 0; p < G; ++p)
+                if (dbg[p].n_other || dbg[p].new_node != 0xFFFFFFFFu) at.push_back((uint32_t)p);
+            allele_strings<BITS>(oc, at.data(), dbg.data(), true, (uint32_t)at.size(), pool, off);
+            texts[1] = pp::DEBUG_HEADER;
+            size_t k = 0;
+            for (uint32_t ci = 0; ci < c->n_contigs; ++ci)
+                for (uint64_t p = c->off[ci]; p < c->off[ci + 1]; ++p) {
+                    const uint8_t* al = (k < at.size() && at[k] == p) ? pool.data() + off[k++] : nullptr;
+                    rows.add(texts[1], names[ci], p - c->off[ci], dbg[p], al);
+                }
+        }
+        if (STS) {                                          // the runs, then the lines contig by contig
+            static const char* const word[6] = {"low_depth", "none", "multiple", "too_close", "kept", "changed"};
+            auto text = [](std::string& o, uint8_t s) {
+                if (s > 5) return false;
+                o += word[s];
+                return true;
+            };
+            const int rc = runs_text(c, vp.sts + key_bytes, names, text, &texts[2]);
+            if (rc) return rc;
+        }
+        if (DEP) {
+            auto text = [](std::string& o, unsigned long long t) {
+                pp::depth_text(o, t);
+                return true;
+            };
+            const int rc = runs_text(c, (const unsigned long long*)vp.sts, names, text, &texts[3]);
+            if (rc) return rc;
+        }
+    }
     *err_out = st.err;
     res->out_len = st.out_len;
     res->n_aln_used = st.n_used;
@@ -131,6 +243,16 @@ int run(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm
         if (res->total_depth) memcpy(res->total_depth, tdepth.data(), c->n_contigs * 8);
     }
     return PP_OK;
+}
+
+// The run instance of the k_tile instance the product runs for these reports (tile_kernel<BITS>() in polish_kernels.cu).
+using RunFn = int (*)(const pp_contigs*, const pp_alignments*, const pp_polish_params*, pp_polish_result*, int, bool, bool, uint64_t*,
+                      const char* const*, std::string*);
+template <int BITS> RunFn run_for(unsigned reports) {
+    static const RunFn k[8] = {run<BITS, false, false, false>, run<BITS, false, false, true>, run<BITS, false, true, false>,
+                               run<BITS, false, true, true>, run<BITS, true, false, false>, run<BITS, true, false, true>,
+                               run<BITS, true, true, false>, run<BITS, true, true, true>};
+    return k[(reports & R_CHANGES ? 4 : 0) + (reports & R_STATUS ? 2 : 0) + (reports & R_DEPTH ? 1 : 0)];
 }
 
 }  // namespace
@@ -151,14 +273,57 @@ extern "C" void emu_last_layout(uint32_t* n_bins, uint32_t* n_slots, uint32_t* n
     if (tile_order) std::copy(g_last_tile_order.begin(), g_last_tile_order.end(), tile_order);
 }
 
-// The polish kernels on the CPU.  grid_tiles = CTAs of k_tile (they share tiles through the ticket, like on the device).
-extern "C" int emu_polish(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,
-                          unsigned long long* err_code) {
+// The polish kernels on the CPU with per-position reports.  grid_tiles = CTAs of k_tile (they share tiles through the ticket, like on
+// the device).  reports = R_* bits; names = the contigs' names.  texts[0 .. 3] (free with emu_free) receive, for each report asked
+// for, the bytes `polish --changes`, `--debug`, `--status-bed` and `--depth-bedgraph` write; the others are null.  101: the runs are
+// malformed.
+extern "C" int emu_polish_reports(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res,
+                                  int grid_tiles, unsigned reports, const char* const* names, unsigned long long* err_code, char** texts) {
     init_comp_table();
     uint64_t err = 0;
-    int rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, false, &err) : run<8>(c, a, prm, res, grid_tiles, false, &err);
+    std::string t[N_REPORTS];
+    auto go = [&](bool global_k) {
+        for (std::string& x : t) x.clear();
+        const RunFn f = a->seq_bits == 4 ? run_for<4>(reports) : run_for<8>(reports);
+        return f(c, a, prm, res, grid_tiles, global_k, reports & R_DEBUG, &err, names, t);
+    };
+    int rc = go(false);
     g_last_global_k = rc == 100;
-    if (rc == 100) rc = a->seq_bits == 4 ? run<4>(c, a, prm, res, grid_tiles, true, &err) : run<8>(c, a, prm, res, grid_tiles, true, &err);
+    if (rc == 100) rc = go(true);
     if (err_code) *err_code = err;
+    for (int i = 0; i < N_REPORTS; ++i) texts[i] = reports >> i & 1 ? strdup(t[i].c_str()) : nullptr;
     return rc;
 }
+
+// The polish kernels on the CPU with no report.  This entry point keeps the signature it has always had: a library built from this file
+// has the same name in build/ as one built from an earlier revision, and a binding of either must be able to call the other's
+// emu_polish without corrupting its arguments.
+extern "C" int emu_polish(const pp_contigs* c, const pp_alignments* a, const pp_polish_params* prm, pp_polish_result* res, int grid_tiles,
+                          unsigned long long* err_code) {
+    char* texts[N_REPORTS];
+    return emu_polish_reports(c, a, prm, res, grid_tiles, 0, nullptr, err_code, texts);
+}
+
+// depth_tenths(x[i]) into tenths[i]; returns the first i whose depth text (pp::depth_text of the tenths) is not snprintf("%.1f", x[i]),
+// or n when there is none.
+extern "C" uint64_t emu_depth_tenths(const double* x, uint64_t n, unsigned long long* tenths) {
+    std::string t;
+    char want[512];
+    for (uint64_t i = 0; i < n; ++i) {
+        tenths[i] = depth_tenths(x[i]);
+        t.clear();
+        pp::depth_text(t, tenths[i]);
+        snprintf(want, sizeof want, "%.1f", x[i]);
+        if (t != want) return i;
+    }
+    return n;
+}
+
+// pp::depth_text of each key, one per line (free with emu_free)
+extern "C" char* emu_depth_text(const unsigned long long* tenths, uint64_t n) {
+    std::string t;
+    for (uint64_t i = 0; i < n; ++i) { pp::depth_text(t, tenths[i]); t += '\n'; }
+    return strdup(t.c_str());
+}
+
+extern "C" void emu_free(void* p) { free(p); }

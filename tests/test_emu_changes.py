@@ -3,7 +3,7 @@ formatter against the oracle's --debug TSV filtered to its `changed` rows, byte 
 import pytest
 
 import polypolish_b200 as pp
-from tests import emu_changes_lib, emu_lib, fuzzgen
+from tests import emu_lib, fuzzgen
 from tests.test_emu_depth_boundary import HALF_BELOW, HALF_ON, MIN_DEPTH_BELOW, MIN_DEPTH_ON, _seq_sum, write_case
 
 # k of the alignments over the probed position in two SAM orders: the reference's depth is 3.25 (printed "3.2") in the first and
@@ -21,7 +21,7 @@ def check_changes(oracle, fa, sams, grid_tiles=2, **opts):
     exp = oracle.polish(fa, sams, debug=True, **opts)
     f = pp.load_fasta(fa)
     p = pp.pack_sams(f, sams, careful=opts.get("careful", False))
-    r = emu_changes_lib.polish(f, p, grid_tiles=grid_tiles, **opts)
+    r = emu_lib.polish(f, p, grid_tiles=grid_tiles, changes=True, **opts)
     assert "error" not in r, r
     assert emu_lib.fasta_bytes(f, r["sequences"]) == exp["fasta"]
     assert r["changes"] == changed_rows(exp["debug_tsv"])

@@ -7,13 +7,13 @@ import numpy as np
 import pytest
 
 import polypolish_b200 as pp
-from tests import depthgen, emu_depth_lib, emu_lib, endgen, fuzzgen, statusgen, walkgen
+from tests import depthgen, emu_lib, endgen, fuzzgen, statusgen, walkgen
 
 
 # ---- depth_tenths and the host's text ----------------------------------------------------------------------------------------------
 def check_tenths(x):
     x = np.asarray(x, dtype=np.float64)
-    t, bad = emu_depth_lib.depth_tenths(x)
+    t, bad = emu_lib.depth_tenths(x)
     assert bad == len(x), "depth_tenths(%r) = %d, snprintf says %s" % (x[bad], t[bad], "%.1f" % x[bad])
     assert t.tolist() == [depthgen.tenths(v) for v in x.tolist()]
 
@@ -27,7 +27,7 @@ def neighbours(x):
 def test_tenths_twentieths():
     """Every n/20 up to 10^5 (all the decimal ties x.x5 and the tenths), each with the doubles either side of it."""
     x = neighbours(np.arange(0, 2_000_001, dtype=np.float64) / 20.0)
-    t, bad = emu_depth_lib.depth_tenths(x)
+    t, bad = emu_lib.depth_tenths(x)
     assert bad == len(x), "depth_tenths(%r) = %d, snprintf says %s" % (x[bad], t[bad], "%.1f" % x[bad])
 
 
@@ -35,7 +35,7 @@ def test_tenths_exact_ties():
     """x.25 and x.75 are exact in binary: round half to even gives x.2 and x.8, never x.3 or x.7."""
     x = np.array([n + f for n in (0, 1, 2, 7, 100, 12345, 2 ** 31, 2 ** 32 - 1) for f in (0.25, 0.75)], dtype=np.float64)
     check_tenths(neighbours(x))
-    t, _ = emu_depth_lib.depth_tenths(np.array([0.25, 0.75, 1.25, 1.75]))
+    t, _ = emu_lib.depth_tenths(np.array([0.25, 0.75, 1.25, 1.75]))
     assert t.tolist() == [2, 8, 12, 18]
 
 
@@ -58,7 +58,7 @@ def test_depth_text():
     """The host formats the key with integers only: tenths / 10, ".", tenths % 10 - what snprintf("%.1f") prints of that many tenths."""
     keys = [0, 1, 9, 10, 11, 99, 100, 101, 12345, 10 ** 10 + 7, (1 << 36) - 1]
     want = b"".join(b"%.1f\n" % (k / 10) for k in keys[:-2]) + b"1000000000.7\n6871947673.5\n"
-    assert emu_depth_lib.depth_text(np.array(keys, np.uint64)) == want
+    assert emu_lib.depth_text(np.array(keys, np.uint64)) == want
 
 
 # ---- the emulated kernels against the oracle ---------------------------------------------------------------------------------------
@@ -66,7 +66,7 @@ def check_depth(oracle, fa, sams, grid_tiles=2, with_changes=False, with_status=
     exp = oracle.polish(fa, sams, debug=True, **opts)
     f = pp.load_fasta(fa)
     p = pp.pack_sams(f, sams, careful=opts.get("careful", False))
-    r = emu_depth_lib.polish(f, p, grid_tiles=grid_tiles, with_changes=with_changes, with_status=with_status, **opts)
+    r = emu_lib.polish(f, p, grid_tiles=grid_tiles, depth=True, changes=with_changes, status=with_status, **opts)
     assert "error" not in r, r
     assert emu_lib.fasta_bytes(f, r["sequences"]) == exp["fasta"]
     assert r["bedgraph"] == depthgen.bedgraph_from_debug_tsv(exp["debug_tsv"])
@@ -76,8 +76,8 @@ def check_depth(oracle, fa, sams, grid_tiles=2, with_changes=False, with_status=
     # depth off: the same FASTA and statistics.  The total depth adds the walk's sum where depth mode walked and the fixed-point
     # estimate elsewhere (within n 2^-41 of each other per position), in atomics of no fixed order: equal to rounding
     plain = emu_lib.polish(f, p, grid_tiles=grid_tiles, **opts)
-    assert plain["sequences"] == r["sequences"] and plain["changed"] == r["changed"] and plain["zero_depth"] == r["zero"]
-    assert all(math.isclose(a, b, rel_tol=1e-9, abs_tol=1e-9) for a, b in zip(plain["total_depth"], r["tdepth"])), (plain["total_depth"], r["tdepth"])
+    assert plain["sequences"] == r["sequences"] and plain["changed"] == r["changed"] and plain["zero_depth"] == r["zero_depth"]
+    assert all(math.isclose(a, b, rel_tol=1e-9, abs_tol=1e-9) for a, b in zip(plain["total_depth"], r["total_depth"])), (plain["total_depth"], r["total_depth"])
     return r, exp
 
 

@@ -11,7 +11,7 @@ import sys
 import pytest
 
 import polypolish_b200 as pp
-from tests import emu_lib, emu_ring_lib, ringgen as rg
+from tests import emu_lib, ringgen as rg
 from tests.test_emu_changes import changed_rows
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -25,9 +25,9 @@ def child(case_dir, mode, grid):
     p = pp.pack_sams(f, sams)
     if mode == "plain":
         r = emu_lib.polish(f, p, grid_tiles=grid)
-        r["layout"] = {k: v.tolist() for k, v in emu_ring_lib.last_layout().items()}
+        r["layout"] = {k: v.tolist() for k, v in emu_lib.last_layout().items()}
     else:
-        r = emu_ring_lib.polish_report(f, p, grid_tiles=grid)
+        r = emu_lib.polish(f, p, grid_tiles=grid, changes=True, debug=True)
     r["seq_bits"] = p.view.seq_bits
     if "sequences" in r:                                    # (else an input error: the parent reports it)
         r["fasta"] = emu_lib.fasta_bytes(f, r.pop("sequences"))

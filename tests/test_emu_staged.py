@@ -12,7 +12,7 @@ import pytest
 
 import polypolish_b200 as pp
 from polypolish_b200 import api
-from tests import emu_lib, emu_ring_lib, stagedgen as sg
+from tests import emu_lib, stagedgen as sg
 from tests.test_emu_changes import changed_rows
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -40,9 +40,9 @@ def child(case_dir, mode, grid):
         queued.value = 0
         r = emu_lib.polish(f, p, grid_tiles=grid)
         r["n_queued"] = queued.value
-        r["layout"] = {k: v.tolist() for k, v in emu_ring_lib.last_layout().items()}
+        r["layout"] = {k: v.tolist() for k, v in emu_lib.last_layout().items()}
     else:
-        r = emu_ring_lib.polish_report(f, p, grid_tiles=grid)
+        r = emu_lib.polish(f, p, grid_tiles=grid, changes=True, debug=True)
     r["seq_bits"] = p.view.seq_bits
     if "sequences" in r:
         r["fasta"] = emu_lib.fasta_bytes(f, r.pop("sequences"))

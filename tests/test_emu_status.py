@@ -4,14 +4,14 @@ only."""
 import pytest
 
 import polypolish_b200 as pp
-from tests import emu_lib, emu_status_lib, endgen, fuzzgen, statusgen
+from tests import emu_lib, endgen, fuzzgen, statusgen
 
 
 def check_status(oracle, fa, sams, grid_tiles=2, with_changes=False, **opts):
     exp = oracle.polish(fa, sams, debug=True, **opts)
     f = pp.load_fasta(fa)
     p = pp.pack_sams(f, sams, careful=opts.get("careful", False))
-    r = emu_status_lib.polish(f, p, grid_tiles=grid_tiles, with_changes=with_changes, **opts)
+    r = emu_lib.polish(f, p, grid_tiles=grid_tiles, status=True, changes=with_changes, **opts)
     assert "error" not in r, r
     assert emu_lib.fasta_bytes(f, r["sequences"]) == exp["fasta"]
     assert r["bed"] == statusgen.bed_from_debug_tsv(exp["debug_tsv"])
