@@ -446,6 +446,42 @@ int pp_filter_polish_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* ass
 void pp_free(void* p);
 
 /* ------------------------------------------------------------------------------------------------------
+ * Batches: many whole commands, one after the other on each of several contexts (`polypolish batch`).
+ * ---------------------------------------------------------------------------------------------------- */
+#define PP_BATCH_POLISH 0         /* pp_polish_files(ctx, assembly, sams, n_sams, &params, debug, ...)                          */
+#define PP_BATCH_FILTER_POLISH 1  /* pp_filter_polish_files(ctx, assembly, in1, in2, out1, out2, orientation, low, high, ...)   */
+typedef struct {                  /* one job: the arguments of the call its kind names; what that call does not take is ignored */
+  int32_t kind;                   /* PP_BATCH_POLISH | PP_BATCH_FILTER_POLISH */
+  const char* assembly;
+  const char* const* sams;        /* polish: the SAM files (may be NULL when n_sams == 0) */
+  int32_t n_sams;
+  const char *in1, *in2, *out1, *out2, *orientation;   /* filter-polish: out1 / out2 may be NULL, orientation NULL = "auto" */
+  double low, high;
+  pp_polish_params params;
+  const char *debug, *changes, *status_bed, *vcf, *depth_bedgraph;   /* report files, NULL or "" = off; debug: polish only */
+  const char* output;             /* the polished FASTA (what the command prints to stdout), created only when the job succeeds */
+} pp_batch_job;
+typedef struct {
+  int32_t rc;                     /* the job's return code; PP_ERR_CUDA also for a job that was not run (see below) */
+  int32_t context;                /* index into ctxs of the context it ran on, -1 = not run */
+  double wall_ms;                 /* host wall time of the job */
+  char* log;                      /* the job's verbose log (what the call prints to stderr), NUL-terminated; free with pp_free */
+  char* error;                    /* rc != 0: the job's error message (pp_last_error), else NULL; free with pp_free */
+} pp_batch_result;
+typedef void (*pp_batch_done_fn)(int job, const pp_batch_result* result, void* user);
+/* Runs jobs[0..n_jobs) on ctxs[0..n_ctx): one host thread per context takes the next job in order and runs it whole on its context
+ * (a job never spans contexts).  Every per-job setting of a context (the report files, the log sink) is set for the job and cleared
+ * after it; what the caller set on the contexts (pp_set_parser, ...) holds for every job.  The FASTA of a job goes to job.output only
+ * when the job succeeded; report files and filtered SAM files are written exactly as the job's own call writes them.  With verbose,
+ * each job's log is captured into its result instead of going to stderr.  on_done (may be NULL) is called on the CALLING thread, in job
+ * order, as soon as that job and every job before it have finished.  A job that fails with PP_ERR_CUDA stops its context's thread (the
+ * device may be unusable); jobs no remaining thread can take get rc PP_ERR_CUDA, context -1 and an error naming the context and the job
+ * that failed.  Jobs are numbered from 1 in messages.  A failing job does not stop the others.  Returns PP_OK when every job succeeded,
+ * PP_ERR_INPUT when any failed (their results say why), PP_ERR_ARG for bad arguments (then no job ran and no result is set). */
+int pp_batch_files(pp_ctx* const* ctxs, int n_ctx, const pp_batch_job* jobs, int n_jobs, pp_batch_result* results, int verbose,
+                   pp_batch_done_fn on_done, void* user);
+
+/* ------------------------------------------------------------------------------------------------------
  * Synthetic inputs (measurement / test support; SURVEY.md §8d).  Deterministic in `seed`.
  * ---------------------------------------------------------------------------------------------------- */
 typedef struct {

@@ -5,7 +5,7 @@ CLI built next to it.  This package is only the thin ctypes mirror of that ABI u
 it contains no compute and no fallback: importing works anywhere, but every compute call raises unless the
 CUDA library is built and an H100 (compute capability 9.0) is visible.
 """
-from .api import (Context, PolypolishError, filter_sams, lib, lib_path, load_fasta, pack_sams, polish,  # noqa: F401
+from .api import (Context, PolypolishError, batch, filter_sams, lib, lib_path, load_fasta, pack_sams, polish,  # noqa: F401
                   polish_files)
 
 __version__ = "0.6.1-b200"

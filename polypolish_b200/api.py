@@ -925,3 +925,78 @@ def filter_polish_files_multi(assembly, in1, in2, out1=None, out2=None, orientat
         L.pp_free(out)
         return data
     return _with_contexts(devices, contexts, parser, run)
+
+
+# ---- batches (csrc/batch.cpp) ----------------------------------------------------------------------------------------
+PP_BATCH_POLISH, PP_BATCH_FILTER_POLISH = 0, 1
+_BATCH_KINDS = {"polish": PP_BATCH_POLISH, "filter-polish": PP_BATCH_FILTER_POLISH}
+
+
+class BatchJob(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("assembly", C.c_char_p), ("sams", C.POINTER(C.c_char_p)), ("n_sams", C.c_int32),
+                ("in1", C.c_char_p), ("in2", C.c_char_p), ("out1", C.c_char_p), ("out2", C.c_char_p), ("orientation", C.c_char_p),
+                ("low", C.c_double), ("high", C.c_double), ("params", PolishParams), ("debug", C.c_char_p), ("changes", C.c_char_p),
+                ("status_bed", C.c_char_p), ("vcf", C.c_char_p), ("depth_bedgraph", C.c_char_p), ("output", C.c_char_p)]
+
+
+class BatchResult(C.Structure):
+    _fields_ = [("rc", C.c_int32), ("context", C.c_int32), ("wall_ms", C.c_double), ("log", C.c_void_p), ("error", C.c_void_p)]
+
+
+def _path(x):
+    return str(x).encode() if x else None
+
+
+def batch(jobs, devices=None, contexts=None, verbose=False, parser=None):
+    """pp_batch_files: whole `polish` / `filter-polish` jobs, one job per context at a time, over one context per entry of `devices`
+    (entries may repeat; default [0]) or over the given `contexts`.  A job is a dict with "kind" ("polish" or "filter-polish"),
+    "output" (the polished FASTA, written only when the job succeeds) and the keyword arguments of Context.polish_files /
+    Context.filter_polish_files ("assembly", "sams", "debug", "changes", "status", "vcf", "depth_bedgraph", "in1", "in2", "out1",
+    "out2", "orientation", "low", "high", and the polish options).  parser: None leaves the contexts' parsers as they are, 0 / 1 sets
+    every context's.  Returns one dict per job, in job order: ok, rc, error (the job's message, or None), log (what the job's own call
+    prints with verbose), context (the index of the context it ran on, -1 = not run) and wall_ms."""
+    L = lib()
+    L.pp_batch_files.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(BatchJob), C.c_int, C.POINTER(BatchResult), C.c_int,
+                                 C.c_void_p, C.c_void_p]
+    arr = (BatchJob * max(1, len(jobs)))()
+    keep = []
+    for b, job in zip(arr, jobs):
+        job = dict(job)
+        kind = job.pop("kind")
+        if kind not in _BATCH_KINDS:
+            raise ValueError("job kind %r: 'polish' or 'filter-polish'" % (kind,))
+        b.kind = _BATCH_KINDS[kind]
+        b.assembly = _path(job.pop("assembly"))
+        sams = [str(x).encode() for x in job.pop("sams", [])]
+        b.sams = (C.c_char_p * max(1, len(sams)))(*sams)
+        b.n_sams = len(sams)
+        keep.append(b.sams)
+        for key in ("in1", "in2", "out1", "out2", "debug", "changes", "vcf", "depth_bedgraph", "output"):
+            setattr(b, key, _path(job.pop(key, None)))
+        b.status_bed = _path(job.pop("status", None))
+        b.orientation = job.pop("orientation", "auto").encode()
+        b.low, b.high = job.pop("low", 0.1), job.pop("high", 99.9)
+        b.params = _params(**job)
+    res = (BatchResult * max(1, len(jobs)))()
+
+    def run(ctxs, arr_ctx):
+        if parser is not None:
+            for c in ctxs:
+                c.set_parser(parser)
+        rc = L.pp_batch_files(arr_ctx, len(ctxs), arr, len(jobs), res, int(verbose), None, None)
+        if rc == PP_ERR_ARG:
+            raise PolypolishError(rc, "pp_batch_files: bad arguments")
+        out = []
+        for r in res[:len(jobs)]:
+            text = {k: C.string_at(getattr(r, k)).decode("utf-8", "replace") if getattr(r, k) else None for k in ("log", "error")}
+            for k in ("log", "error"):
+                L.pp_free(getattr(r, k))
+            out.append(dict(ok=r.rc == PP_OK, rc=r.rc, error=text["error"], log=text["log"] or "", context=r.context, wall_ms=r.wall_ms))
+        return out
+    ctxs = contexts if contexts is not None else [Context(d) for d in (devices if devices is not None else [0])]
+    try:
+        return run(ctxs, (C.c_void_p * len(ctxs))(*[c.h for c in ctxs]))
+    finally:
+        if contexts is None:
+            for c in ctxs:
+                c.close()

@@ -18,7 +18,7 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-Wall,-Wno-unus
           "-fmad=false"]   # IEEE double semantics: no FMA contraction anywhere near the vote
 
 LIB_SOURCES = ["polish_kernels.cu", "filter_kernels.cu", "tok_kernels.cu", "fasta.cpp", "sam_pack.cpp", "filter_pack.cpp",
-               "host_api.cpp", "synth.cpp", "shard.cpp"]
+               "host_api.cpp", "batch.cpp", "synth.cpp", "shard.cpp"]
 CLI_SOURCES = ["cli_main.cpp"]
 
 

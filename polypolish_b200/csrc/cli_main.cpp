@@ -11,6 +11,7 @@
 // positions only), --status-bed F (polish, filter-polish: every position's --debug status as BED runs), --vcf F (polish,
 // filter-polish: the polish's edits to the draft as VCF records that rebuild the polished FASTA), --depth-bedgraph F (polish,
 // filter-polish: every position's --debug depth as bedGraph runs).
+// Additive command: `polypolish batch MANIFEST` runs many `polish` / `filter-polish` command lines in one process (pp_batch_files).
 // All compute happens in libpolypolish_b200.so on the GPU.
 #include <cstdio>
 #include <unistd.h>
@@ -18,6 +19,9 @@
 #include <cstring>
 #include <algorithm>
 #include <chrono>
+#include <fstream>
+#include <map>
+#include <sstream>
 #include <string>
 #include <vector>
 
@@ -38,8 +42,10 @@ static const char* BANNER =
     exit(1);
 }
 
+static std::string usage_where;          // `batch`: "manifest line N: " while a job line is parsed, so that its errors name the line
+
 [[noreturn]] static void usage_error(const std::string& text) {      // clap argument errors exit with 2
-    fprintf(stderr, "error: %s\n\nFor more information, try '--help'.\n", text.c_str());
+    fprintf(stderr, "error: %s%s\n\nFor more information, try '--help'.\n", usage_where.c_str(), text.c_str());
     exit(2);
 }
 
@@ -47,7 +53,8 @@ static void help() {                      // `polypolish`, `polypolish -h`: the 
     fputs(BANNER, stdout);
     puts("\nshort-read polishing of long-read assemblies\ngithub.com/rrwick/Polypolish\n");
     puts("Usage: polypolish <COMMAND>\n");
-    puts("Commands:\n  filter  filter paired-end alignments based on insert size\n  polish  polish a long-read assembly using short-read alignments\n");
+    puts("Commands:\n  filter  filter paired-end alignments based on insert size\n  polish  polish a long-read assembly using short-read alignments\n"
+         "  batch   run many polish / filter-polish jobs listed in a manifest, one job per GPU at a time (H100 build only)\n");
     puts("Options:\n  -h, --help     Print help\n  -V, --version  Print version");
 }
 
@@ -166,7 +173,7 @@ struct Args {
     std::vector<Token> tok;
     size_t i = 0;
     pp_polish_params prm{0.2, 0.5, 10, 5, 0};
-    std::string debug, changes, status_bed, vcf, depth_bedgraph, in1, in2, out1, out2, orientation = "auto";
+    std::string debug, changes, status_bed, vcf, depth_bedgraph, in1, in2, out1, out2, orientation = "auto", output;
     double low = 0.1, high = 99.9;
     int device = 0, gpus = 1;
     bool quiet = false, host_parse = false;
@@ -263,6 +270,198 @@ static std::vector<pp_ctx*> open_contexts(const Args& g) {
     _exit(0);
 }
 
+// The own options of `polish` and `filter-polish` (after -h / -V, which print and exit), and their required arguments: shared by the
+// commands themselves and by the job lines of `batch`.
+static bool polish_own(const std::string& a, Args& g) {
+    if (a == "--debug") { g.debug = g.value("--debug <DEBUG>"); return true; }
+    return polish_option(a, g);
+}
+static void polish_required(const Args& g) {
+    if (g.pos.empty()) usage_error("the following required arguments were not provided:\n  <ASSEMBLY>");
+}
+static bool filter_polish_own(const std::string& a, Args& g) {
+    return filter_option(a, g) || polish_option(a, g) || gpu_count_option(a, g);
+}
+static void filter_polish_required(const Args& g) {
+    if (g.in1.empty() || g.in2.empty() || g.pos.size() != 1)
+        usage_error("the following required arguments were not provided:\n  --in1 <IN1>\n  --in2 <IN2>\n  <ASSEMBLY>");
+}
+
+static void help_batch() {
+    puts("run many polish / filter-polish jobs listed in a manifest in one process, one job per GPU at a time (H100 build only)\n");
+    puts("Usage: polypolish batch [OPTIONS] <MANIFEST>\n");
+    puts("Arguments:");
+    puts("  <MANIFEST>  One job per line: `polish` or `filter-polish`, then that command's own arguments, plus --output <FILE>");
+    puts("\nOptions:");
+    puts("      --device <N>  First GPU [default: 0]");
+    puts("      --gpus <N>    GPUs to run jobs on, one job per GPU at a time [default: 1]");
+    puts("      --quiet       Print only the failed jobs");
+    puts("      --host-parse  Parse the SAM text on the host (every job)");
+    puts("  -h, --help        Print help");
+    puts("\nManifest: blank lines and lines starting with '#' are ignored; fields are separated by spaces or tabs, so a path cannot "
+         "contain whitespace; relative paths are relative to the working directory.  --output <FILE> (required) receives the polished "
+         "FASTA the command would print to stdout, and is created only when the job succeeds.  --device, --gpus, --gpu-count, --quiet "
+         "and --host-parse belong on the batch command line.  No two output files (FASTA, reports, --out1 / --out2) may be the same, "
+         "and no job may read a file another job writes.  Log on stderr: one block per job in manifest order; exit status 1 if any job "
+         "failed.");
+}
+
+// One job line of a manifest, parsed as its command would parse it.
+struct BatchJob {
+    int line = 0;
+    std::string cmd;
+    Args g;
+};
+
+// "a//b/./c/../d" relative to the working directory -> "/cwd/a/b/d": two names of one file that differ only lexically compare equal.
+static std::string lexical_path(const std::string& p) {
+    std::string full = p;
+    if (p.empty() || p[0] != '/') {
+        char cwd[4096];
+        full = std::string(getcwd(cwd, sizeof cwd) ? cwd : ".") + "/" + p;
+    }
+    std::vector<std::string> parts;
+    std::stringstream ss(full);
+    for (std::string item; std::getline(ss, item, '/');) {
+        if (item.empty() || item == ".") continue;
+        if (item == "..") { if (!parts.empty()) parts.pop_back(); continue; }
+        parts.push_back(item);
+    }
+    std::string out;
+    for (auto& x : parts) out += "/" + x;
+    return out.empty() ? "/" : out;
+}
+
+// The manifest, every line checked before any CUDA call: usage errors (exit 2) name the line.
+static std::vector<BatchJob> read_manifest(const std::string& path) {
+    std::ifstream in(path, std::ios::binary);
+    if (!in) usage_error("unable to read the manifest \"" + path + "\"");
+    std::vector<BatchJob> jobs;
+    std::string text;
+    for (int line = 1; std::getline(in, text); ++line) {
+        if (!text.empty() && text.back() == '\r') text.pop_back();
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : text + " ") {
+            if (c == ' ' || c == '\t') { if (!cur.empty()) f.push_back(cur); cur.clear(); }
+            else cur += c;
+        }
+        if (f.empty() || f[0][0] == '#') continue;
+        usage_where = "manifest line " + std::to_string(line) + ": ";
+        const bool polish = f[0] == "polish";
+        if (!polish && f[0] != "filter-polish") usage_error("unrecognized command '" + f[0] + "' (a job is `polish` or `filter-polish`)");
+        std::vector<char*> argv = {(char*)"polypolish"};
+        for (auto& x : f) argv.push_back(&x[0]);
+        BatchJob j;
+        j.line = line;
+        j.cmd = f[0];
+        j.g = parse_args((int)argv.size(), argv.data(), "ivmd", true, polish, [polish](const std::string& a, Args& g) {
+            if (a == "--output") { g.output = g.value("--output <FILE>"); return true; }
+            if (a == "--device" || a == "--gpus" || a == "--gpu-count" || a == "--quiet" || a == "--host-parse")
+                usage_error("'" + a + "' applies to every job: it belongs on the `polypolish batch` command line");
+            if (a == "-h" || a == "--help" || a == "-V" || a == "--version") usage_error("unexpected argument '" + a + "' found");
+            return polish ? polish_own(a, g) : filter_polish_own(a, g);
+        });
+        if (polish) polish_required(j.g);
+        else filter_polish_required(j.g);
+        if (j.g.output.empty()) usage_error("the following required arguments were not provided:\n  --output <FILE>");
+        jobs.push_back(std::move(j));
+    }
+    usage_where.clear();
+    if (in.bad()) usage_error("unable to read the manifest \"" + path + "\"");
+    if (jobs.empty()) usage_error("the manifest \"" + path + "\" has no jobs");
+    // every file a job writes is written by that job alone, and read by no job
+    std::map<std::string, int> written;
+    for (const BatchJob& j : jobs) {
+        usage_where = "manifest line " + std::to_string(j.line) + ": ";
+        const Args& g = j.g;
+        for (const std::string* o : {&g.output, &g.debug, &g.changes, &g.status_bed, &g.vcf, &g.depth_bedgraph, &g.out1, &g.out2}) {
+            if (o->empty()) continue;
+            auto [it, fresh] = written.emplace(lexical_path(*o), j.line);
+            if (!fresh) usage_error("the output file '" + *o + "' is also written by " + (it->second == j.line ? "this line" : "line " + std::to_string(it->second)));
+        }
+    }
+    for (const BatchJob& j : jobs) {
+        usage_where = "manifest line " + std::to_string(j.line) + ": ";
+        std::vector<std::string> inputs = j.g.pos;
+        if (!j.g.in1.empty()) inputs.push_back(j.g.in1);
+        if (!j.g.in2.empty()) inputs.push_back(j.g.in2);
+        for (const std::string& x : inputs) {
+            auto it = written.find(lexical_path(x));
+            if (it != written.end() && it->second != j.line)
+                usage_error("the input file '" + x + "' is written by line " + std::to_string(it->second) + " (jobs may run in any order)");
+        }
+    }
+    usage_where.clear();
+    return jobs;
+}
+
+// What the on_done callback of `batch` prints with: one block per job, in manifest order.
+struct BatchPrint {
+    const std::vector<BatchJob>* jobs;
+    int first_gpu;
+    bool quiet;
+    int failed = 0;
+};
+
+static void print_job(int i, const pp_batch_result* r, void* user) {
+    BatchPrint& p = *(BatchPrint*)user;
+    const BatchJob& j = (*p.jobs)[(size_t)i];
+    p.failed += r->rc != PP_OK;
+    if (p.quiet && r->rc == PP_OK) return;
+    std::string gpu = r->context >= 0 ? "GPU " + std::to_string(p.first_gpu + r->context) : "not run";
+    fprintf(stderr, "[job %d/%zu] manifest line %d: %s -> %s (%s)\n", i + 1, p.jobs->size(), j.line, j.cmd.c_str(), j.g.output.c_str(), gpu.c_str());
+    if (!p.quiet && r->log) fputs(r->log, stderr);
+    if (r->rc == PP_OK) fprintf(stderr, "Finished!\n");
+    else fprintf(stderr, "Error: %s\n", r->error ? r->error : "unknown error");
+    if (!p.quiet) fputc('\n', stderr);
+    fflush(stderr);
+}
+
+[[noreturn]] static void run_batch(int argc, char** argv) {
+    Args g = parse_args(argc, argv, "", true, true, [](const std::string& a, Args&) {
+        if (a == "-h" || a == "--help") { help_batch(); exit(0); }
+        if (a == "-V" || a == "--version") { puts("Polypolish-batch v0.6.1"); exit(0); }
+        return false;
+    });
+    if (g.pos.empty()) usage_error("the following required arguments were not provided:\n  <MANIFEST>");
+    if (g.pos.size() > 1) usage_error("unexpected argument '" + g.pos[1] + "' found");
+    const std::vector<BatchJob> jobs = read_manifest(g.pos[0]);
+    // every job's arguments, as pp_batch_files takes them (the strings stay in `jobs`)
+    std::vector<std::vector<const char*>> sams(jobs.size());
+    std::vector<pp_batch_job> bj(jobs.size());
+    auto opt = [](const std::string& s) { return s.empty() ? nullptr : s.c_str(); };
+    for (size_t i = 0; i < jobs.size(); ++i) {
+        const Args& a = jobs[i].g;
+        pp_batch_job& b = bj[i];
+        memset(&b, 0, sizeof b);
+        b.kind = jobs[i].cmd == "polish" ? PP_BATCH_POLISH : PP_BATCH_FILTER_POLISH;
+        b.assembly = a.pos[0].c_str();
+        if (b.kind == PP_BATCH_POLISH)
+            for (size_t k = 1; k < a.pos.size(); ++k) sams[i].push_back(a.pos[k].c_str());
+        b.sams = sams[i].data();
+        b.n_sams = (int)sams[i].size();
+        b.in1 = opt(a.in1); b.in2 = opt(a.in2); b.out1 = opt(a.out1); b.out2 = opt(a.out2); b.orientation = a.orientation.c_str();
+        b.low = a.low; b.high = a.high; b.params = a.prm;
+        b.debug = opt(a.debug); b.changes = opt(a.changes); b.status_bed = opt(a.status_bed); b.vcf = opt(a.vcf);
+        b.depth_bedgraph = opt(a.depth_bedgraph);
+        b.output = a.output.c_str();
+    }
+    std::vector<pp_ctx*> ctxs = open_contexts(g);           // (g names no report file: those are each job's own)
+    for (pp_ctx* c : ctxs) pp_set_parser(c, g.host_parse ? 1 : 0);
+    if (!g.quiet)
+        fprintf(stderr, "Starting Polypolish batch (H100 build %s, %zu job%s, %d GPU%s)\n\n", pp_version(), jobs.size(), jobs.size() > 1 ? "s" : "",
+                g.gpus, g.gpus > 1 ? "s" : "");
+    BatchPrint bp{&jobs, g.device, g.quiet};
+    std::vector<pp_batch_result> res(jobs.size());
+    const int rc = pp_batch_files(ctxs.data(), g.gpus, bj.data(), (int)bj.size(), res.data(), g.quiet ? 0 : 1, print_job, &bp);
+    if (rc == PP_ERR_ARG) quit_with_error("pp_batch_files: bad arguments");
+    mark("batch done");
+    if (!g.quiet) fprintf(stderr, "Batch finished: %zu job%s, %d failed\n", jobs.size(), jobs.size() > 1 ? "s" : "", bp.failed);
+    fflush(stderr);
+    _exit(bp.failed ? 1 : 0);                             // as finish(): the kernel reclaims the contexts
+}
+
 int main(int argc, char** argv) {
     mark("main");
     if (argc < 2) { help(); return 2; }
@@ -275,10 +474,9 @@ int main(int argc, char** argv) {
         Args g = parse_args(argc, argv, "ivmd", true, true, [](const std::string& a, Args& g) {
             if (a == "-h" || a == "--help") { help_polish(); exit(0); }
             if (a == "-V" || a == "--version") { puts("Polypolish-polish v0.6.1"); exit(0); }
-            if (a == "--debug") { g.debug = g.value("--debug <DEBUG>"); return true; }
-            return polish_option(a, g);
+            return polish_own(a, g);
         });
-        if (g.pos.empty()) usage_error("the following required arguments were not provided:\n  <ASSEMBLY>");
+        polish_required(g);
         std::vector<pp_ctx*> ctxs = open_contexts(g);
         if (!g.quiet) fprintf(stderr, "Starting Polypolish polish (H100 build %s, %d GPU%s)\n\n", pp_version(), g.gpus, g.gpus > 1 ? "s" : "");
         std::vector<const char*> sams;
@@ -310,10 +508,9 @@ int main(int argc, char** argv) {
                 puts("Options: those of `filter` (--out1 / --out2 optional: written only when given) and of `polish` (except --debug)");
                 exit(0);
             }
-            return filter_option(a, g) || polish_option(a, g) || gpu_count_option(a, g);
+            return filter_polish_own(a, g);
         });
-        if (g.in1.empty() || g.in2.empty() || g.pos.size() != 1)
-            usage_error("the following required arguments were not provided:\n  --in1 <IN1>\n  --in2 <IN2>\n  <ASSEMBLY>");
+        filter_polish_required(g);
         std::vector<pp_ctx*> ctxs = open_contexts(g);
         if (!g.quiet) fprintf(stderr, "Starting Polypolish filter + polish (H100 build %s%s)\n\n", pp_version(), g.gpus > 1 ? (", " + std::to_string(g.gpus) + " GPUs").c_str() : "");
         const int rc = pp_filter_polish_files_multi(ctxs.data(), g.gpus, g.pos[0].c_str(), g.in1.c_str(), g.in2.c_str(),
@@ -321,5 +518,6 @@ int main(int argc, char** argv) {
                                                     g.orientation.c_str(), g.low, g.high, &g.prm, &out, &n, g.quiet ? 0 : 1);
         finish(ctxs, rc, out, n, g.quiet);
     }
+    if (cmd == "batch") run_batch(argc, argv);
     usage_error("unrecognized subcommand '" + cmd + "'");
 }

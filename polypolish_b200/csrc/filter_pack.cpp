@@ -133,22 +133,22 @@ int pp::check_filter_args(pp_ctx* ctx, const char* in1, const char* in2, const c
 }
 
 // get_insert_size_thresholds' log (filter.rs:168-186)
-static void log_thresholds(const char* orientation, const pp_filter_params* prm, const pp_filter_result* res) {
+static void log_thresholds(pp_ctx* ctx, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res) {
     static const char* nm[4] = {"fr", "rf", "ff", "rr"};
-    for (int i = 0; i < 4; ++i) fprintf(stderr, "%s: %s pairs\n", nm[i], pp::thousands(res->pairs[i]).c_str());
-    fprintf(stderr, "\n%s correct orientation: %s\n\n", prm->orientation < 0 ? "Automatically determined" : "User-specified",
+    for (int i = 0; i < 4; ++i) pp_log(ctx, "%s: %s pairs\n", nm[i], pp::thousands(res->pairs[i]).c_str());
+    pp_log(ctx, "\n%s correct orientation: %s\n\n", prm->orientation < 0 ? "Automatically determined" : "User-specified",
             res->orientation < 4 ? nm[res->orientation] : orientation);
-    fprintf(stderr, "Low threshold:  %u\nHigh threshold: %u\n\n", res->low, res->high);
+    pp_log(ctx, "Low threshold:  %u\nHigh threshold: %u\n\n", res->low, res->high);
 }
 
-void pp_filter_log(const char* in1, const char* in2, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res,
-                   const pp_filter_file_stats* fs) {
+void pp_filter_log(pp_ctx* ctx, const char* in1, const char* in2, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res,
+             const pp_filter_file_stats* fs) {
     const char* ins[2] = {in1, in2};
-    for (int k = 0; k < 2; ++k) fprintf(stderr, "%s: %s alignments\n", ins[k], pp::thousands(fs->alignments[k]).c_str());
-    log_thresholds(orientation, prm, res);
+    for (int k = 0; k < 2; ++k) pp_log(ctx, "%s: %s alignments\n", ins[k], pp::thousands(fs->alignments[k]).c_str());
+    log_thresholds(ctx, orientation, prm, res);
     for (int k = 0; k < 2; ++k)
-        fprintf(stderr, "Filtering %s:\n  %s pass\n  %s fail\n\n", ins[k], pp::thousands(fs->pass[k]).c_str(), pp::thousands(fs->fail[k]).c_str());
-    fprintf(stderr, "Alignments before filtering: %s\nAlignments after filtering:  %s\n\n", pp::thousands(fs->alignments[0] + fs->alignments[1]).c_str(),
+        pp_log(ctx, "Filtering %s:\n  %s pass\n  %s fail\n\n", ins[k], pp::thousands(fs->pass[k]).c_str(), pp::thousands(fs->fail[k]).c_str());
+    pp_log(ctx, "Alignments before filtering: %s\nAlignments after filtering:  %s\n\n", pp::thousands(fs->alignments[0] + fs->alignments[1]).c_str(),
             pp::thousands(fs->pass[0] + fs->pass[1]).c_str());
 }
 
@@ -169,10 +169,10 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
         int rc = pp_filter_files_device(ctx, in1, in2, out1, out2, &prm, &res, &fs, nullptr);
         if (rc == PP_OK) {
             if (verbose) {
-                pp_filter_log(in1, in2, orientation, &prm, &res, &fs);
-                fprintf(stderr, "device text path: %.3f ms (SAM to HBM %.3f ms, filtered SAM to files %.3f ms), %u kernels; filter kernels %.3f ms\n", fs.total_ms,
+                pp_filter_log(ctx, in1, in2, orientation, &prm, &res, &fs);
+                pp_log(ctx, "device text path: %.3f ms (SAM to HBM %.3f ms, filtered SAM to files %.3f ms), %u kernels; filter kernels %.3f ms\n", fs.total_ms,
                         fs.h2d_ms, fs.d2h_ms, fs.launches, res.timing.total_ms);
-                fprintf(stderr, "  phases (wall ms): upload+index+parse %.1f, intern+verify+emit %.1f, filter %.1f, output offsets %.1f, output bytes %.1f, download+write %.1f\n",
+                pp_log(ctx, "  phases (wall ms): upload+index+parse %.1f, intern+verify+emit %.1f, filter %.1f, output offsets %.1f, output bytes %.1f, download+write %.1f\n",
                         fs.phase_ms[0], fs.phase_ms[1], fs.phase_ms[2], fs.phase_ms[3], fs.phase_ms[4], fs.phase_ms[5]);
             }
             return PP_OK;
@@ -188,7 +188,7 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
     std::string err;
     for (int k = 0; k < 2; ++k) {
         if (!load_mate(m[k], names, err)) return pp_ctx_fail(ctx, PP_ERR_INPUT, err.c_str());
-        if (verbose) fprintf(stderr, "%s: %s alignments\n", m[k].path.c_str(), pp::thousands(m[k].name_id.size()).c_str());
+        if (verbose) pp_log(ctx, "%s: %s alignments\n", m[k].path.c_str(), pp::thousands(m[k].name_id.size()).c_str());
         if (m[0].name_id.empty() && (k == 0 || m[1].name_id.empty()))      // alignments.is_empty() filter.rs:141-143
             return pp_ctx_fail(ctx, PP_ERR_INPUT, ("no alignments found in \"" + m[k].path + "\"").c_str());
     }
@@ -205,7 +205,7 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
     res.pass2 = pass2.data();
     int rc = pp_filter(ctx, &fm[0], &fm[1], &prm, &res);
     if (rc != PP_OK) return rc;
-    if (verbose) log_thresholds(orientation, &prm, &res);
+    if (verbose) log_thresholds(ctx, orientation, &prm, &res);
     uint64_t before = fm[0].n + fm[1].n, after = 0;
     const uint8_t* passes[2] = {pass1.data(), pass2.data()};
     for (int k = 0; k < 2; ++k) {
@@ -213,11 +213,11 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
         if (!write_filtered(m[k], passes[k], outs[k], np, nf))
             return pp_ctx_fail(ctx, PP_ERR_IO, ("unable to write alignments to \"" + std::string(outs[k]) + "\"").c_str());
         after += np;
-        if (verbose) fprintf(stderr, "Filtering %s:\n  %s pass\n  %s fail\n\n", m[k].path.c_str(), pp::thousands(np).c_str(), pp::thousands(nf).c_str());
+        if (verbose) pp_log(ctx, "Filtering %s:\n  %s pass\n  %s fail\n\n", m[k].path.c_str(), pp::thousands(np).c_str(), pp::thousands(nf).c_str());
     }
     if (verbose) {
-        fprintf(stderr, "Alignments before filtering: %s\nAlignments after filtering:  %s\n\n", pp::thousands(before).c_str(), pp::thousands(after).c_str());
-        fprintf(stderr, "device path: %.3f ms, %u kernels\n", res.timing.total_ms, res.timing.launches);
+        pp_log(ctx, "Alignments before filtering: %s\nAlignments after filtering:  %s\n\n", pp::thousands(before).c_str(), pp::thousands(after).c_str());
+        pp_log(ctx, "device path: %.3f ms, %u kernels\n", res.timing.total_ms, res.timing.launches);
     }
     return PP_OK;
 }
@@ -244,10 +244,10 @@ extern "C" int pp_filter_files_multi(pp_ctx* const* ctxs, int n_ctx, const char*
         pp_filter_file_stats fs;
         rc = pp_filter_files_device_multi(ctxs, n_ctx, in1, in2, out1, out2, &prm, c, &res, &fs, nullptr);
         if (rc == PP_OK && verbose) {
-            pp_filter_log(in1, in2, orientation, &prm, &res, &fs);
-            fprintf(stderr, "device text path over %d GPUs: %.3f ms (SAM to HBM %.3f ms on the slowest GPU, filtered SAM to files %.3f ms), %u kernels\n", n_ctx,
+            pp_filter_log(ctx, in1, in2, orientation, &prm, &res, &fs);
+            pp_log(ctx, "device text path over %d GPUs: %.3f ms (SAM to HBM %.3f ms on the slowest GPU, filtered SAM to files %.3f ms), %u kernels\n", n_ctx,
                     fs.total_ms, fs.h2d_ms, fs.d2h_ms, fs.launches);
-            fprintf(stderr, "  phases (wall ms): upload+index+parse+intern %.1f, records to their name's GPU %.1f, filter %.1f\n", fs.phase_ms[0],
+            pp_log(ctx, "  phases (wall ms): upload+index+parse+intern %.1f, records to their name's GPU %.1f, filter %.1f\n", fs.phase_ms[0],
                     fs.phase_ms[1], fs.phase_ms[2]);
         }
     }

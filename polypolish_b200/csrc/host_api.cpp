@@ -7,6 +7,7 @@
 // pp_polish() / pp_filter() on the device.  There is no CPU fallback for that work.
 #include <chrono>
 #include <cmath>
+#include <cstdarg>
 #include <fcntl.h>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -41,6 +42,27 @@ std::string qscore_text(double identity) {
 }  // namespace
 
 extern "C" void pp_free(void* p) { free(p); }
+
+void pp_log(pp_ctx* ctx, const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    if (ctx && ctx->log) {
+        va_list aq;
+        va_copy(aq, ap);
+        const int n = vsnprintf(nullptr, 0, fmt, aq);
+        va_end(aq);
+        if (n > 0) {
+            std::string& s = *ctx->log;
+            const size_t at = s.size();
+            s.resize(at + (size_t)n + 1);
+            vsnprintf(&s[at], (size_t)n + 1, fmt, ap);
+            s.resize(at + (size_t)n);
+        }
+    } else {
+        vfprintf(stderr, fmt, ap);
+    }
+    va_end(ap);
+}
 
 // One shard on one GPU (run by its own host thread when there are several).
 struct ShardJob {
@@ -474,9 +496,9 @@ static int job_error(pp_ctx* ctx, const Load& ld) {
     return PP_OK;
 }
 
-// print_seq_to_stdout polish.rs:196-203, contigs in input order (polish.rs:147-152), with the per-contig statistics on stderr
+// print_seq_to_stdout polish.rs:196-203, contigs in input order (polish.rs:147-152), with the per-contig statistics in ctx's log
 // (polish.rs:205-226) when verbose.
-static std::string assemble(const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>& jobs, int verbose) {
+static std::string assemble(pp_ctx* ctx, const pp_fasta* fa, const pp_contigs& contigs, const std::vector<ShardJob>& jobs, int verbose) {
     // where each input contig's polished bases are: (job, local contig)
     std::vector<std::pair<uint32_t, uint32_t>> where(contigs.n_contigs);
     for (uint32_t s = 0; s < jobs.size(); ++s)
@@ -498,14 +520,14 @@ static std::string assemble(const pp_fasta* fa, const pp_contigs& contigs, const
         out += '\n';
         if (verbose) {
             uint64_t len = contigs.off[i + 1] - contigs.off[i];
-            fprintf(stderr, "Polishing %s (%s bp):\n", pp_fasta_name(fa, i), pp::thousands(len).c_str());
-            fprintf(stderr, "  mean read depth: %.1fx\n", j.tdepth[lc] / (double)len);                       // polish.rs:208-210
-            fprintf(stderr, "  %s bp %s a depth of zero (%.4f%% coverage)\n", pp::thousands(j.zero[lc]).c_str(), j.zero[lc] == 1 ? "has" : "have",
+            pp_log(ctx, "Polishing %s (%s bp):\n", pp_fasta_name(fa, i), pp::thousands(len).c_str());
+            pp_log(ctx, "  mean read depth: %.1fx\n", j.tdepth[lc] / (double)len);                       // polish.rs:208-210
+            pp_log(ctx, "  %s bp %s a depth of zero (%.4f%% coverage)\n", pp::thousands(j.zero[lc]).c_str(), j.zero[lc] == 1 ? "has" : "have",
                     100.0 * (double)(len - j.zero[lc]) / (double)len);
-            fprintf(stderr, "  %s %s changed (%.4f%% of total positions)\n", pp::thousands(j.changed[lc]).c_str(),
+            pp_log(ctx, "  %s %s changed (%.4f%% of total positions)\n", pp::thousands(j.changed[lc]).c_str(),
                     j.changed[lc] == 1 ? "position" : "positions", 100.0 * (double)j.changed[lc] / (double)len);
             const double accuracy = 100.0 - 100.0 * (double)j.changed[lc] / (double)len;
-            fprintf(stderr, "  estimated pre-polishing sequence accuracy: %.4f%% (%s)\n\n", accuracy, qscore_text(accuracy).c_str());
+            pp_log(ctx, "  estimated pre-polishing sequence accuracy: %.4f%% (%s)\n\n", accuracy, qscore_text(accuracy).c_str());
         }
     }
     return out;
@@ -688,12 +710,12 @@ struct ReportFile {
     ~ReportFile() { if (f) fclose(f); }
 };
 
-static void print_timing(const Load& ld) {
-    fputs(ld.timing.c_str(), stderr);
+static void print_timing(pp_ctx* ctx, const Load& ld) {
+    pp_log(ctx, "%s", ld.timing.c_str());
     for (uint32_t s = 0; s < ld.jobs.size(); ++s) {
         const ShardJob& j = ld.jobs[s];
         const pp_timing& t = j.res.timing;
-        fprintf(stderr, "GPU job %u: %u contigs, %s alignments; device path %.3f ms (h2d + binning %.3f, goodness/k %.3f, tile %.3f, compact %.3f, d2h %.3f), %u kernels\n",
+        pp_log(ctx, "GPU job %u: %u contigs, %s alignments; device path %.3f ms (h2d + binning %.3f, goodness/k %.3f, tile %.3f, compact %.3f, d2h %.3f), %u kernels\n",
                 s, j.contigs.n_contigs, pp::thousands(j.alns.n_aln).c_str(), t.total_ms, t.stage_ms[6], t.stage_ms[2], t.stage_ms[3],
                 t.stage_ms[4], t.stage_ms[7], t.launches);
     }
@@ -739,10 +761,10 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     pp_contigs contigs;
     pp_fasta_view(fa.get(), &contigs);
     if (verbose) {
-        fprintf(stderr, "Loading assembly\n");
+        pp_log(ctx, "Loading assembly\n");
         for (uint32_t i = 0; i < contigs.n_contigs; ++i)
-            fprintf(stderr, "%s (%s bp)\n", pp_fasta_name(fa.get(), i), pp::thousands(contigs.off[i + 1] - contigs.off[i]).c_str());
-        fprintf(stderr, "\nLoading alignments\n");
+            pp_log(ctx, "%s (%s bp)\n", pp_fasta_name(fa.get(), i), pp::thousands(contigs.off[i + 1] - contigs.off[i]).c_str());
+        pp_log(ctx, "\nLoading alignments\n");
     }
 
     // one job per GPU; with one GPU the job is the whole assembly.  The debug TSV is written from one GPU.
@@ -756,13 +778,13 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
                 : load_device(ctxs, n_shards, fa.get(), contigs, sams, n_sams, prm->careful, ld);
         if (rc == PP_OK) run_jobs(ld.jobs, prm);
         if (rc == PP_OK && data_error(ld.jobs)) rc = PP_TOK_HOST;
-        if (rc == PP_OK && verbose) fputs(ld.log.c_str(), stderr);
+        if (rc == PP_OK && verbose) pp_log(ctx, "%s", ld.log.c_str());
     }
     if (rc == PP_TOK_HOST) {
         if (ff) return PP_TOK_HOST;
         ld = Load();
         rc = load_host(ctxs, n_shards, fa.get(), contigs, sams, n_sams, prm->careful, ld);
-        if (verbose) fputs(ld.log.c_str(), stderr);
+        if (verbose) pp_log(ctx, "%s", ld.log.c_str());
         if (rc == PP_OK) run_jobs(ld.jobs, prm);
         if (rc == PP_OK && data_error(ld.jobs) && ld.jobs.size() > 1) {
             // the message names the read / reference of the offending line: its index in the unsharded arrays is what the packer can
@@ -787,12 +809,12 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
     if (verbose) {
         uint64_t n_used = 0;
         for (const ShardJob& j : ld.jobs) n_used += j.res.n_aln_used;
-        fprintf(stderr, "\nFiltering for high-quality end-to-end alignments%s:\n", prm->careful ? " from reads with only one alignment" : "");
-        fprintf(stderr, "  %s alignments kept\n", pp::thousands(n_used).c_str());
-        fprintf(stderr, "  %s alignments discarded\n\n", pp::thousands(ld.alns.n_aln - n_used).c_str());
+        pp_log(ctx, "\nFiltering for high-quality end-to-end alignments%s:\n", prm->careful ? " from reads with only one alignment" : "");
+        pp_log(ctx, "  %s alignments kept\n", pp::thousands(n_used).c_str());
+        pp_log(ctx, "  %s alignments discarded\n\n", pp::thousands(ld.alns.n_aln - n_used).c_str());
     }
-    const std::string out = assemble(fa.get(), contigs, ld.jobs, verbose);
-    if (verbose) print_timing(ld);
+    const std::string out = assemble(ctx, fa.get(), contigs, ld.jobs, verbose);
+    if (verbose) print_timing(ctx, ld);
     char* buf = (char*)malloc(out.size() + 1);
     if (!buf) return pp_ctx_fail(ctx, PP_ERR_NOMEM, "out of memory");
     memcpy(buf, out.data(), out.size());

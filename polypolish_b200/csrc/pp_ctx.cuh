@@ -82,6 +82,7 @@ struct pp_ctx {
     std::string report_path[F_COUNT];     // pp_set_*_file: the reports the file-level commands also write ("" = none)
     TokState* tok = nullptr;              // SAM tokeniser state (tok_kernels.cu), created on first use
     int parser = 0;                       // pp_set_parser: 0 device tokeniser where possible, 1 host packer only
+    std::string* log = nullptr;           // pp_batch_files: the running job's verbose log goes here instead of stderr (pp_log)
 
     int fail(int code, const std::string& m) { err = m; return code; }
     int fail_cuda(cudaError_t e, const char* what, const char* file, int line) {

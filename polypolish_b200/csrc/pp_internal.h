@@ -106,6 +106,9 @@ struct pp_pack {
 };
 
 int pp_ctx_fail(pp_ctx* ctx, int code, const char* msg);
+// Every verbose line of the file-level calls: printf-style, appended to the context's log sink when pp_batch_files has set one, else
+// written to stderr.
+void pp_log(pp_ctx* ctx, const char* fmt, ...) __attribute__((format(printf, 2, 3)));
 // --debug: the allele strings (k_allele_strings' format, row i at pool[off[i]]) of the last call's records at n global positions
 int pp_polish_debug_strings(pp_ctx* ctx, const uint32_t* pos, uint32_t n, std::vector<uint64_t>& off, std::vector<uint8_t>& pool);
 
@@ -133,6 +136,6 @@ int pp_filter_files_device(pp_ctx* ctx, const char* in1, const char* in2, const 
 int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
                                  const pp_filter_params* prm, const uint64_t* const cuts[2], pp_filter_result* res, pp_filter_file_stats* fs,
                                  pp_fused_polish* fuse);
-// the filter's log on stderr (filter.rs:26-37 and the functions it calls), shared by the one-context and the multi-context calls
-void pp_filter_log(const char* in1, const char* in2, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res,
+// the filter's log (filter.rs:26-37 and the functions it calls) through pp_log, shared by the one-context and the multi-context calls
+void pp_filter_log(pp_ctx* ctx, const char* in1, const char* in2, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res,
                    const pp_filter_file_stats* fs);
