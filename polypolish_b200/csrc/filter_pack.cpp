@@ -152,34 +152,52 @@ void pp_filter_log(pp_ctx* ctx, const char* in1, const char* in2, const char* or
             pp::thousands(fs->pass[0] + fs->pass[1]).c_str());
 }
 
-extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, const char* out1, const char* out2,
-                               const char* orientation, double low, double high, int verbose) {
-    if (!ctx) return PP_ERR_ARG;
+// `polypolish filter` on ctxs[0 .. n_ctx).  The device text path first, where the SAM text never leaves the device between parse and
+// write (tok_kernels.cu): over all the contexts when there are several and both files can be cut between read groups
+// (pp_sam_split_ranges; GPU g filters byte range g of both files, the records meet on the GPU that owns their read name), then on ctxs[0]
+// alone.  Whatever that path does not settle - the host parser asked for, an input that is not a regular file, PP_TOK_HOST (malformed
+// line, empty file, ...) - is done by the host text path, which words the reference's messages.
+extern "C" int pp_filter_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                                     const char* orientation, double low, double high, int verbose) {
+    if (!ctxs || n_ctx < 1 || !ctxs[0]) return PP_ERR_ARG;
+    pp_ctx* ctx = ctxs[0];
+    for (int g = 1; g < n_ctx; ++g)
+        if (!ctxs[g]) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_files_multi: null context");
     if (!in1 || !in2 || !out1 || !out2 || !orientation) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_files: null argument");
     pp_filter_params prm;
     if (int rc = pp::check_filter_args(ctx, in1, in2, out1, out2, orientation, low, high, &prm); rc != PP_OK) return rc;
     pp_filter_result res;
+    auto device = [&](int n, const uint64_t* const* cuts) {
+        memset(&res, 0, sizeof res);
+        pp_filter_file_stats fs;
+        const int rc = pp_filter_files_device(ctxs, n, in1, in2, out1, out2, &prm, cuts, &res, &fs, nullptr);
+        if (rc != PP_OK || !verbose) return rc;
+        pp_filter_log(ctx, in1, in2, orientation, &prm, &res, &fs);
+        if (n == 1) {
+            pp_log(ctx, "device text path: %.3f ms (SAM to HBM %.3f ms, filtered SAM to files %.3f ms), %u kernels; filter kernels %.3f ms\n", fs.total_ms,
+                    fs.h2d_ms, fs.d2h_ms, fs.launches, res.timing.total_ms);
+            pp_log(ctx, "  phases (wall ms): upload+index+parse %.1f, intern+verify+emit %.1f, filter %.1f, output offsets %.1f, output bytes %.1f, download+write %.1f\n",
+                    fs.phase_ms[0], fs.phase_ms[1], fs.phase_ms[2], fs.phase_ms[3], fs.phase_ms[4], fs.phase_ms[5]);
+        } else {
+            pp_log(ctx, "device text path over %d GPUs: %.3f ms (SAM to HBM %.3f ms on the slowest GPU, filtered SAM to files %.3f ms), %u kernels\n", n,
+                    fs.total_ms, fs.h2d_ms, fs.d2h_ms, fs.launches);
+            pp_log(ctx, "  phases (wall ms): upload+index+parse+intern %.1f, records to their name's GPU %.1f, filter %.1f\n", fs.phase_ms[0],
+                    fs.phase_ms[1], fs.phase_ms[2]);
+        }
+        return PP_OK;
+    };
+    if (pp_get_parser(ctx) == 0) {
+        int rc = PP_TOK_HOST;
+        std::vector<uint64_t> cuts[2] = {std::vector<uint64_t>((size_t)n_ctx + 1), std::vector<uint64_t>((size_t)n_ctx + 1)};
+        if (n_ctx > 1 && pp_sam_split_ranges(in1, n_ctx, cuts[0].data()) == PP_OK && pp_sam_split_ranges(in2, n_ctx, cuts[1].data()) == PP_OK) {
+            const uint64_t* c[2] = {cuts[0].data(), cuts[1].data()};
+            rc = device(n_ctx, c);
+        }
+        if (rc == PP_TOK_HOST) rc = device(1, nullptr);
+        if (rc != PP_TOK_HOST) return rc;
+    }
     memset(&res, 0, sizeof res);
     const char* outs[2] = {out1, out2};
-
-    // Fast path: the SAM text never leaves the device between parse and write (tok_kernels.cu).  PP_TOK_HOST = something the
-    // device path leaves to the host code below (malformed line, empty file, ...), which words the reference's messages.
-    if (pp_get_parser(ctx) == 0) {
-        pp_filter_file_stats fs;
-        int rc = pp_filter_files_device(ctx, in1, in2, out1, out2, &prm, &res, &fs, nullptr);
-        if (rc == PP_OK) {
-            if (verbose) {
-                pp_filter_log(ctx, in1, in2, orientation, &prm, &res, &fs);
-                pp_log(ctx, "device text path: %.3f ms (SAM to HBM %.3f ms, filtered SAM to files %.3f ms), %u kernels; filter kernels %.3f ms\n", fs.total_ms,
-                        fs.h2d_ms, fs.d2h_ms, fs.launches, res.timing.total_ms);
-                pp_log(ctx, "  phases (wall ms): upload+index+parse %.1f, intern+verify+emit %.1f, filter %.1f, output offsets %.1f, output bytes %.1f, download+write %.1f\n",
-                        fs.phase_ms[0], fs.phase_ms[1], fs.phase_ms[2], fs.phase_ms[3], fs.phase_ms[4], fs.phase_ms[5]);
-            }
-            return PP_OK;
-        }
-        if (rc != PP_TOK_HOST) return rc;
-        memset(&res, 0, sizeof res);
-    }
 
     MateFile m[2];
     m[0].path = in1;
@@ -222,35 +240,7 @@ extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, co
     return PP_OK;
 }
 
-// `polypolish filter` over several GPUs: GPU g filters byte range g of both files (pp_sam_split_ranges), the records meet on the GPU
-// that owns their read name, the thresholds are reduced across GPUs (tok_kernels.cu).  Whatever that path does not settle - the
-// host parser asked for, an input that is not a regular file, PP_TOK_HOST - is the one-context call's on ctxs[0].
-extern "C" int pp_filter_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
-                                     const char* orientation, double low, double high, int verbose) {
-    if (!ctxs || n_ctx < 1 || !ctxs[0]) return PP_ERR_ARG;
-    pp_ctx* ctx = ctxs[0];
-    for (int g = 1; g < n_ctx; ++g)
-        if (!ctxs[g]) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_files_multi: null context");
-    if (n_ctx == 1 || pp_get_parser(ctx) != 0) return pp_filter_files(ctx, in1, in2, out1, out2, orientation, low, high, verbose);
-    if (!in1 || !in2 || !out1 || !out2 || !orientation) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_files: null argument");
-    pp_filter_params prm;
-    if (int rc = pp::check_filter_args(ctx, in1, in2, out1, out2, orientation, low, high, &prm); rc != PP_OK) return rc;
-    std::vector<uint64_t> cuts[2] = {std::vector<uint64_t>((size_t)n_ctx + 1), std::vector<uint64_t>((size_t)n_ctx + 1)};
-    int rc = PP_TOK_HOST;
-    if (pp_sam_split_ranges(in1, n_ctx, cuts[0].data()) == PP_OK && pp_sam_split_ranges(in2, n_ctx, cuts[1].data()) == PP_OK) {
-        const uint64_t* c[2] = {cuts[0].data(), cuts[1].data()};
-        pp_filter_result res;
-        memset(&res, 0, sizeof res);
-        pp_filter_file_stats fs;
-        rc = pp_filter_files_device_multi(ctxs, n_ctx, in1, in2, out1, out2, &prm, c, &res, &fs, nullptr);
-        if (rc == PP_OK && verbose) {
-            pp_filter_log(ctx, in1, in2, orientation, &prm, &res, &fs);
-            pp_log(ctx, "device text path over %d GPUs: %.3f ms (SAM to HBM %.3f ms on the slowest GPU, filtered SAM to files %.3f ms), %u kernels\n", n_ctx,
-                    fs.total_ms, fs.h2d_ms, fs.d2h_ms, fs.launches);
-            pp_log(ctx, "  phases (wall ms): upload+index+parse+intern %.1f, records to their name's GPU %.1f, filter %.1f\n", fs.phase_ms[0],
-                    fs.phase_ms[1], fs.phase_ms[2]);
-        }
-    }
-    if (rc != PP_TOK_HOST) return rc;
-    return pp_filter_files(ctx, in1, in2, out1, out2, orientation, low, high, verbose);
+extern "C" int pp_filter_files(pp_ctx* ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                               const char* orientation, double low, double high, int verbose) {
+    return pp_filter_files_multi(&ctx, 1, in1, in2, out1, out2, orientation, low, high, verbose);
 }

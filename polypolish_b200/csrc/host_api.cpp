@@ -402,14 +402,13 @@ static int load_fused(pp_ctx* const* ctxs, uint32_t n, const pp_fasta* fa, const
     fuse.fasta = fa; fuse.careful = careful;
     std::vector<uint32_t> owner;
     std::vector<std::vector<uint64_t>> cuts;
-    int rc;
-    if (n == 1) {
-        rc = pp_filter_files_device(ctx, sams[0], sams[1], ff.out1, ff.out2, &ff.prm, &fres, &fs, &fuse);
-    } else {
+    const uint64_t* c[2] = {nullptr, nullptr};
+    int rc = PP_OK;
+    if (n > 1) {
         rc = plan_device_shards(ctxs, n, contigs, sams, 2, ld, owner, cuts);
-        const uint64_t* c[2] = {cuts.size() == 2 ? cuts[0].data() : nullptr, cuts.size() == 2 ? cuts[1].data() : nullptr};
-        if (rc == PP_OK) rc = pp_filter_files_device_multi(ctxs, (int)n, sams[0], sams[1], ff.out1, ff.out2, &ff.prm, c, &fres, &fs, &fuse);
+        if (rc == PP_OK) { c[0] = cuts[0].data(); c[1] = cuts[1].data(); }
     }
+    if (rc == PP_OK) rc = pp_filter_files_device(ctxs, (int)n, sams[0], sams[1], ff.out1, ff.out2, &ff.prm, n > 1 ? c : nullptr, &fres, &fs, &fuse);
     if (rc == PP_OK && fuse.rc == PP_TOK_HOST) rc = PP_TOK_HOST;
     if (rc != PP_OK) return rc;
     static const char* nm[4] = {"fr", "rf", "ff", "rr"};
@@ -424,7 +423,7 @@ static int load_fused(pp_ctx* const* ctxs, uint32_t n, const pp_fasta* fa, const
     ld.alns.n_aln = fuse.n_aln;
     if (n == 1) {
         one_job(ld, ctx, contigs, true);
-        return PP_OK;
+        return pp_tok_finish(ctx);
     }
     snprintf(tmp, sizeof tmp, "filter over %u GPUs (records to the GPU of their read name, thresholds reduced across GPUs): %.3f ms\n", n, fs.total_ms);
     ld.timing += tmp;
@@ -825,17 +824,24 @@ static int polish_files_impl(pp_ctx* const* ctxs, int n_ctx, const char* assembl
 }
 
 // filter::filter (filter.rs:26-37) then polish::polish (polish.rs:26-38) on its output, as one call: same FASTA as running the two
-// commands through intermediate files, which are only written when the caller names them.
-extern "C" int pp_filter_polish_files(pp_ctx* ctx, const char* assembly, const char* in1, const char* in2, const char* out1, const char* out2,
-                                      const char* orientation, double low, double high, const pp_polish_params* prm, char** out_fasta,
-                                      uint64_t* out_len, int verbose) {
-    if (!ctx) return PP_ERR_ARG;
+// commands through intermediate files, which are only written when the caller names them.  Several GPUs of one box (at most 32) each
+// filter and tokenise their byte range of both files, the read names meet on their owner GPU for the filter, the read groups on their
+// contigs' GPUs for the polish; whatever that does not settle runs on ctxs[0] alone.
+extern "C" int pp_filter_polish_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* assembly, const char* in1, const char* in2, const char* out1,
+                                            const char* out2, const char* orientation, double low, double high, const pp_polish_params* prm,
+                                            char** out_fasta, uint64_t* out_len, int verbose) {
+    if (!ctxs || n_ctx < 1 || !ctxs[0]) return PP_ERR_ARG;
+    pp_ctx* ctx = ctxs[0];
+    for (int g = 1; g < n_ctx; ++g)
+        if (!ctxs[g]) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_polish_files_multi: null context");
     if (!in1 || !in2 || !orientation) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_polish_files: null argument");
     FusedFilter ff{{}, orientation, out1, out2};
     int rc = pp::check_filter_args(ctx, in1, in2, out1, out2, orientation, low, high, &ff.prm);
     if (rc != PP_OK) return rc;
     const char* sams[2] = {in1, in2};
-    rc = polish_files_impl(&ctx, 1, assembly, sams, 2, prm, nullptr, out_fasta, out_len, verbose, &ff);
+    rc = PP_TOK_HOST;
+    if (n_ctx > 1 && n_ctx <= 32) rc = polish_files_impl(ctxs, n_ctx, assembly, sams, 2, prm, nullptr, out_fasta, out_len, verbose, &ff);
+    if (rc == PP_TOK_HOST) rc = polish_files_impl(&ctx, 1, assembly, sams, 2, prm, nullptr, out_fasta, out_len, verbose, &ff);
     if (rc != PP_TOK_HOST) return rc;
     // Something the fused device path leaves to the text code (a malformed line, an empty file, host parsing asked for, a data
     // error whose message needs names): the two commands one after the other, through files, exactly like the reference.
@@ -853,26 +859,10 @@ extern "C" int pp_filter_polish_files(pp_ctx* ctx, const char* assembly, const c
     return rc;
 }
 
-// The same over several GPUs of one box: every GPU filters and tokenises its byte range of both files, the read names meet on their
-// owner GPU for the filter, the read groups on their contigs' GPUs for the polish.  More than 32 contexts, and whatever that path does
-// not settle, are the one-context call's on ctxs[0].
-extern "C" int pp_filter_polish_files_multi(pp_ctx* const* ctxs, int n_ctx, const char* assembly, const char* in1, const char* in2, const char* out1,
-                                            const char* out2, const char* orientation, double low, double high, const pp_polish_params* prm,
-                                            char** out_fasta, uint64_t* out_len, int verbose) {
-    if (!ctxs || n_ctx < 1 || !ctxs[0]) return PP_ERR_ARG;
-    pp_ctx* ctx = ctxs[0];
-    for (int g = 1; g < n_ctx; ++g)
-        if (!ctxs[g]) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_polish_files_multi: null context");
-    if (n_ctx == 1 || n_ctx > 32)
-        return pp_filter_polish_files(ctx, assembly, in1, in2, out1, out2, orientation, low, high, prm, out_fasta, out_len, verbose);
-    if (!in1 || !in2 || !orientation) return pp_ctx_fail(ctx, PP_ERR_ARG, "pp_filter_polish_files: null argument");
-    FusedFilter ff{{}, orientation, out1, out2};
-    int rc = pp::check_filter_args(ctx, in1, in2, out1, out2, orientation, low, high, &ff.prm);
-    if (rc != PP_OK) return rc;
-    const char* sams[2] = {in1, in2};
-    rc = polish_files_impl(ctxs, n_ctx, assembly, sams, 2, prm, nullptr, out_fasta, out_len, verbose, &ff);
-    if (rc != PP_TOK_HOST) return rc;
-    return pp_filter_polish_files(ctx, assembly, in1, in2, out1, out2, orientation, low, high, prm, out_fasta, out_len, verbose);
+extern "C" int pp_filter_polish_files(pp_ctx* ctx, const char* assembly, const char* in1, const char* in2, const char* out1, const char* out2,
+                                      const char* orientation, double low, double high, const pp_polish_params* prm, char** out_fasta,
+                                      uint64_t* out_len, int verbose) {
+    return pp_filter_polish_files_multi(&ctx, 1, assembly, in1, in2, out1, out2, orientation, low, high, prm, out_fasta, out_len, verbose);
 }
 
 static int set_report_file(pp_ctx* ctx, int which, const char* path) {

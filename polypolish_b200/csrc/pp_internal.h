@@ -116,7 +116,9 @@ int pp_polish_debug_strings(pp_ctx* ctx, const uint32_t* pos, uint32_t n, std::v
 struct pp_filter_file_stats {
     uint64_t alignments[2], pass[2], fail[2], text_bytes[2], out_bytes[2];
     float h2d_ms, d2h_ms, total_ms;
-    float phase_ms[6];     // wall: 0 upload+index+parse, 1 intern+verify+emit, 2 filter proper, 3 output lengths+scan, 4 output bytes, 5 download+write
+    // wall: 0 upload+index+parse, 1 intern+verify+emit, 2 filter proper, 3 output lengths+scan, 4 output bytes, 5 download+write; over
+    // several contexts 0 upload+index+parse+intern, 1 records to their name's context, 2 filter proper
+    float phase_ms[6];
     uint32_t launches;
 };
 // filter + polish without the intermediate files: the request to tokenise the resident texts for polish, and what came of it
@@ -127,15 +129,15 @@ struct pp_fused_polish {
     uint64_t n_aln;
     int rc;                // PP_OK: the filtered alignments are the resident dataset; PP_TOK_HOST: the host text path must do it
 };
-int pp_filter_files_device(pp_ctx* ctx, const char* in1, const char* in2, const char* out1, const char* out2, const pp_filter_params* prm,
-                           pp_filter_result* res, pp_filter_file_stats* fs, pp_fused_polish* fuse);
-// The same over several contexts: context g reads bytes [cuts[f][g], cuts[f][g + 1]) of file f (cut between read groups), and the
-// records meet on the context that owns their read name.  With `fuse` every context then tokenises its ranges for polish
-// (pp_tok_set_ranges) with the verdicts as ZP flags, ready for pp_tok_exchange_finish.  fs and fuse->stats are sums over the
-// contexts; errors are reported on ctxs[0].  PP_OK, PP_TOK_HOST (the one-context call must do it) or an error.
-int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
-                                 const pp_filter_params* prm, const uint64_t* const cuts[2], pp_filter_result* res, pp_filter_file_stats* fs,
-                                 pp_fused_polish* fuse);
+// `polypolish filter` with the SAM text handled on the device (tok_kernels.cu), on one context or several.  With `cuts`, context g reads
+// bytes [cuts[f][g], cuts[f][g + 1]) of file f (cut between read groups); `cuts` may be null only when n_ctx is 1, and that context then
+// reads the whole files.  out1 / out2 may be null (not written).  With `fuse` every context then tokenises its text for polish with the
+// verdicts as ZP flags; the caller finishes the dataset (pp_tok_finish on one context, pp_tok_exchange_finish on several).  fs and
+// fuse->stats are sums over the contexts; errors are reported on ctxs[0].  PP_OK, PP_TOK_HOST (a smaller call or the host path must do
+// it) or an error.
+int pp_filter_files_device(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                           const pp_filter_params* prm, const uint64_t* const cuts[2], pp_filter_result* res, pp_filter_file_stats* fs,
+                           pp_fused_polish* fuse);
 // the filter's log (filter.rs:26-37 and the functions it calls) through pp_log, shared by the one-context and the multi-context calls
 void pp_filter_log(pp_ctx* ctx, const char* in1, const char* in2, const char* orientation, const pp_filter_params* prm, const pp_filter_result* res,
                    const pp_filter_file_stats* fs);

@@ -1490,7 +1490,7 @@ static int ftok_lines(pp_ctx* ctx, TokState* T, int which, const uint8_t* text, 
 
 struct TokFilterBufs {                 // device buffers of the filter text path, kept in the tokeniser state
     DevBuf lines[2], tmp[2], mate[2], table, out, status, passkeep;
-    DevBuf fx_refs, fx_stage, fx_rx, fx_owner, fx_home;   // pp_filter_files_multi: see there
+    DevBuf fx_refs, fx_stage, fx_rx, fx_owner, fx_home;   // the filter over several contexts: see filter_exchange
 };
 
 static void free_filter_bufs(TokFilterBufs* b) {
@@ -1506,217 +1506,9 @@ __global__ void __launch_bounds__(256) k_apply_pass(uint8_t* __restrict__ flags,
     if (i < n && !pass[i]) flags[i] |= PP_FLAG_ZPFAIL;
 }
 
-// `polypolish filter` with the SAM text handled on the device.  PP_OK, PP_TOK_HOST (the host path must do it) or an error
-// (the filter's own: no usable pairs, ambiguous orientation; I/O; CUDA).  out1 / out2 may be null (no filtered SAM is written).
-// With `fuse`: the two texts, still resident, are then tokenised for `polish` (pp_tok_*) with the filter's verdict taking the
-// place of the ZP:Z:fail tag the reference would have written and re-read (filter.rs:334-342, alignment.rs:72-74): the resident
-// dataset is what `polish` would load from the filtered files.  fuse->rc = PP_OK / PP_TOK_HOST for that second part.
-int pp_filter_files_device(pp_ctx* ctx, const char* in1, const char* in2, const char* out1, const char* out2, const pp_filter_params* prm_in,
-                           pp_filter_result* res, pp_filter_file_stats* fs, pp_fused_polish* fuse) {
-    CK(cudaSetDevice(ctx->device));
-    TokState* T = nullptr;
-    int rc = tok_state(ctx, &T);
-    if (rc) return rc;
-    if (!T->fbufs) T->fbufs = new TokFilterBufs();
-    TokFilterBufs& B = *T->fbufs;
-    cudaStream_t s = ctx->stream;
-    const char* ins[2] = {in1, in2};
-    const char* outs[2] = {out1, out2};
-    memset(fs, 0, sizeof *fs);
-    const auto t_begin = std::chrono::steady_clock::now();
-    auto t_mark = t_begin;
-    auto lap = [&](int i) { const auto now = std::chrono::steady_clock::now(); fs->phase_ms[i] += std::chrono::duration<float, std::milli>(now - t_mark).count(); t_mark = now; };
-
-    CK(B.status.ensure(sizeof(FStatus)));
-    FStatus* d_st = B.status.as<FStatus>();
-    FStatus h_st;
-    h_st.first_bad[0] = h_st.first_bad[1] = ~0ull; h_st.collision = 0; h_st.pad = 0;
-    CK(cudaMemcpyAsync(d_st, &h_st, sizeof h_st, cudaMemcpyHostToDevice, s));
-    CK(cudaStreamSynchronize(s));
-
-    // ---- both texts into HBM; the second streams in while the first is indexed and parsed
-    FileDev fd[2];
-    uint32_t launches = 0;
-    float h2d_ms = 0;
-    if (T->pf.active && (T->pf.path != in1 || T->pf.strip)) { if (T->pf.th.joinable()) T->pf.th.join(); T->pf.active = false; }
-    for (int k = 0; k < 2; ++k) {
-        rc = prefetch_wait(ctx, T, ins[k], false);
-        if (rc != PP_OK) return rc;
-        const int buf = T->pf.buf;
-        const uint64_t n = T->pf.n;
-        const bool unterminated = n > 0 && T->pf.last != '\n';
-        h2d_ms += T->pf.ms;
-        fs->text_bytes[k] = n;
-        if (k == 0) {
-            rc = prefetch_start(ctx, T, ins[1], false);
-            if (rc != PP_OK) return rc;
-        }
-        rc = ftok_lines(ctx, T, k, T->text[buf].as<uint8_t>(), n, unterminated, B.lines[k], B.tmp[k], d_st, &fd[k], &launches);
-        if (rc != PP_OK) {
-            if (T->pf.active) { if (T->pf.th.joinable()) T->pf.th.join(); T->pf.active = false; }
-            return rc;
-        }
-    }
-    CK(cudaMemcpyAsync(T->h_tot + 0, fd[0].s_al + fd[0].n_lines, 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(T->h_tot + 1, fd[1].s_al + fd[1].n_lines, 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(&h_st, d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    CK(cudaGetLastError());
-    const uint64_t n_al[2] = {T->h_tot[0], T->h_tot[1]};
-    fs->alignments[0] = n_al[0]; fs->alignments[1] = n_al[1];
-    if (h_st.first_bad[0] != ~0ull || h_st.first_bad[1] != ~0ull) return PP_TOK_HOST;
-    if (n_al[0] == 0 || n_al[1] == 0) return PP_TOK_HOST;               // "no alignments found in ..." is worded by the host path
-    if (n_al[0] >= 0x7FFFFFFFull || n_al[1] >= 0x7FFFFFFFull) return PP_TOK_HOST;
-    lap(0);
-
-    // ---- intern QNAMEs and RNAMEs
-    uint64_t cap = 1024;
-    while (cap < 3 * (n_al[0] + n_al[1]) + 1024) cap <<= 1;
-    if (cap > (1ull << 31)) return PP_TOK_HOST;
-    TRY_ALLOC(B.table.ensure(cap * 16));
-    InternTable tb;
-    tb.key = B.table.as<unsigned long long>(); tb.rep = tb.key + cap; tb.mask = (uint32_t)(cap - 1);
-    CK(cudaMemsetAsync(tb.key, 0, cap * 8, s));
-    CK(cudaMemsetAsync(tb.rep, 0xFF, cap * 8, s));
-    for (int k = 0; k < 2; ++k)
-        k_ftok_intern<<<(unsigned)((fd[k].n_lines + TK_LINE_THREADS - 1) / TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(fd[k], k, tb, d_st);
-    Mate mates[2];
-    for (int k = 0; k < 2; ++k) {
-        k_ftok_verify<<<(unsigned)((fd[k].n_lines + TK_LINE_THREADS - 1) / TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(fd[0], fd[1], k, tb, d_st);
-        const size_t na = (size_t)n_al[k];
-        TRY_ALLOC(B.mate[k].ensure(na * 17 + 5 * 256));
-        uint8_t* mb = B.mate[k].as<uint8_t>();
-        auto up = [](size_t v) { return (v + 255) & ~size_t(255); };
-        MateOut mo;
-        mo.name_id = (uint32_t*)mb; mo.contig = (uint32_t*)(mb + up(na * 4)); mo.ref_start = (uint32_t*)(mb + 2 * up(na * 4));
-        mo.ref_end = (uint32_t*)(mb + 3 * up(na * 4)); mo.flags = mb + 4 * up(na * 4);
-        k_ftok_emit<<<(unsigned)((fd[k].n_lines + TK_LINE_THREADS - 1) / TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(fd[k], mo);
-        mates[k].name_id = mo.name_id; mates[k].contig = mo.contig; mates[k].ref_start = mo.ref_start; mates[k].ref_end = mo.ref_end;
-        mates[k].flags = mo.flags; mates[k].cnt = nullptr; mates[k].head = nullptr; mates[k].next = nullptr; mates[k].pass = nullptr;
-        mates[k].n = (uint32_t)na;
-    }
-    launches += 6;
-    CK(cudaMemcpyAsync(&h_st, d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    CK(cudaGetLastError());
-    if (h_st.collision) return PP_TOK_HOST;
-    lap(1);
-
-    // ---- the filter proper (filter_kernels.cu), flags stay on the device
-    pp_filter_params prm = *prm_in;
-    prm.n_names = cap;
-    res->pass1 = nullptr; res->pass2 = nullptr;
-    const uint8_t* d_pass[2] = {nullptr, nullptr};
-    uint64_t np[2] = {0, 0};
-    CK(cudaEventRecord(ctx->ev[0], s));
-    rc = pp_filter_core(ctx, mates, &prm, res, d_pass, np);
-    if (rc != PP_OK) return rc;
-    launches += res->timing.launches;
-    lap(2);
-
-    // ---- output text, file by file: lengths -> offsets -> bytes -> the output file
-    float d2h_ms = 0;
-    for (int k = 0; k < 2; ++k) {
-        fs->pass[k] = np[k];
-        fs->fail[k] = n_al[k] - np[k];
-        if (!outs[k]) continue;
-        const uint64_t nl = fd[k].n_lines;
-        DevBuf& offs = B.table;                                                 // the intern table is done with: reuse it
-        CK(offs.ensure((nl + 2) * 8));
-        unsigned long long* out_off = offs.as<unsigned long long>();
-        k_ftok_outlen<<<(unsigned)((nl + 1 + TK_LINE_THREADS - 1) / TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(fd[k], d_pass[k], out_off);
-        size_t cub_bytes = 0;
-        CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, out_off, out_off, (int64_t)(nl + 1)));
-        CK(T->cub.ensure(cub_bytes + 256));
-        {
-            size_t tbb = T->cub.cap;
-            CK(cub::DeviceScan::ExclusiveSum(T->cub.p, tbb, out_off, out_off, (int64_t)(nl + 1), s));
-        }
-        CK(cudaMemcpyAsync(T->h_tot, out_off + nl, 8, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        const uint64_t out_n = T->h_tot[0];
-        lap(3);
-        TRY_ALLOC(B.out.ensure(out_n + 64));
-        k_ftok_copy<<<(unsigned)((nl * 32 + 255) / 256), 256, 0, s>>>(fd[k], d_pass[k], out_off, B.out.as<uint8_t>());
-        CK(cudaStreamSynchronize(s));
-        CK(cudaGetLastError());
-        launches += 4;
-        lap(4);
-        // A regular file gets its final size up front and is filled in parallel (shared mapping / pwrite at offsets).  Anything
-        // else - a FIFO, >(gzip ...), /dev/stdout into a pipe, /dev/null - cannot be truncated or written at offsets: it is
-        // streamed in order with write(), like the reference's BufWriter (filter.rs:296-349).
-        struct stat osb;
-        const bool special = stat(outs[k], &osb) == 0 && !S_ISREG(osb.st_mode);
-        const int ofd = special ? open(outs[k], O_WRONLY) : open(outs[k], O_RDWR | O_CREAT | O_TRUNC, 0666);
-        if (ofd < 0) return ctx->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + outs[k] + "\"");
-        const auto t0 = std::chrono::steady_clock::now();
-        int cuda_err = 0;
-        int wrc = PP_OK;
-        bool stream_out = special;
-        if (out_n && !stream_out && ftruncate(ofd, (off_t)out_n) != 0) stream_out = true;
-        if (out_n && stream_out) {
-            wrc = download_stream(ctx->device, T, B.out.as<uint8_t>(), ofd, out_n, &cuda_err);
-        } else if (out_n) {
-            // Stores into a mapping cannot report "no space left" (they raise SIGBUS), so the mapping is only used when the
-            // file system has room to spare; otherwise pwrite() reports the error like the reference does (filter.rs:307-311).
-            struct statvfs vfs;
-            const bool roomy = fstatvfs(ofd, &vfs) == 0 && (uint64_t)vfs.f_bavail * (uint64_t)vfs.f_frsize > 2 * out_n + (64ull << 20);
-            void* map = roomy ? mmap(nullptr, (size_t)out_n, PROT_READ | PROT_WRITE, MAP_SHARED, ofd, 0) : MAP_FAILED;
-            if (map == MAP_FAILED) map = nullptr;
-            wrc = download_file(ctx->device, T, B.out.as<uint8_t>(), ofd, (uint8_t*)map, out_n, &cuda_err);
-            if (map && munmap(map, (size_t)out_n) != 0 && wrc == PP_OK) wrc = PP_ERR_IO;
-        }
-        if (close(ofd) != 0 && wrc == PP_OK) wrc = PP_ERR_IO;
-        d2h_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-        if (wrc == PP_ERR_IO) return ctx->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + outs[k] + "\"");
-        if (wrc == PP_ERR_CUDA) return ctx->fail_cuda((cudaError_t)cuda_err, "filtered SAM download", __FILE__, __LINE__);
-        lap(5);
-        fs->out_bytes[k] = out_n;
-    }
-    fs->h2d_ms = h2d_ms;
-    fs->d2h_ms = d2h_ms;
-    fs->launches = launches;
-    if (fuse) {
-        // the verdicts move out of the context's scratch buffer (the tokeniser uses it), then both texts are tokenised in place
-        CK(B.passkeep.ensure(n_al[0] + n_al[1] + 64));
-        uint8_t* keep = B.passkeep.as<uint8_t>();
-        CK(cudaMemcpyAsync(keep, d_pass[0], n_al[0], cudaMemcpyDeviceToDevice, s));
-        CK(cudaMemcpyAsync(keep + n_al[0], d_pass[1], n_al[1], cudaMemcpyDeviceToDevice, s));
-        CK(cudaStreamSynchronize(s));
-        fuse->rc = PP_TOK_HOST;
-        int bits = 4;
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            rc = pp_tok_begin(ctx, fuse->fasta, fuse->careful, bits);
-            if (rc != PP_OK) return rc;
-            T->expect_total = fd[0].n + fd[1].n;
-            memset(fuse->stats, 0, sizeof fuse->stats);
-            for (int k = 0; k < 2 && rc == PP_OK; ++k) {
-                rc = tok_process(ctx, T, fd[k].text, fd[k].n, fd[k].unterminated != 0, &fuse->stats[k]);
-                if (rc == PP_OK && fuse->stats[k].alignments != n_al[k]) rc = PP_TOK_HOST;      // (cannot happen: same lines, same rule)
-            }
-            if (rc == PP_TOK_NEED8 && bits == 4) { bits = 8; continue; }
-            if (rc == PP_TOK_NEED8) rc = PP_TOK_HOST;
-            if (rc < 0) return rc;
-            if (rc == PP_OK) {
-                const uint64_t n = n_al[0] + n_al[1];
-                k_apply_pass<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(ctx->b[B_FLAGS].as<uint8_t>(), keep, n);
-                CK(cudaStreamSynchronize(s));
-                CK(cudaGetLastError());
-                rc = pp_tok_finish(ctx);
-                if (rc < 0) return rc;
-                fuse->n_aln = n;
-            }
-            fuse->rc = rc;
-            break;
-        }
-    }
-    fs->total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
-    return PP_OK;
-}
-
 // =====================================================================================================================
-// `polypolish filter` over several GPUs (pp_filter_files_multi).  GPU g reads byte range g of both files (cut between read groups,
-// so `filter-polish` can hand the same ranges to the polish tokeniser), indexes, parses and interns its lines as above.
+// `polypolish filter` over several GPUs (pp_filter_files_device, n_ctx > 1).  GPU g reads byte range g of both files (cut between read
+// groups, so `filter-polish` can hand the same ranges to the polish tokeniser), indexes, parses and interns its lines as above.
 // A record's verdict (alignment_pass_qc, filter.rs:352-377) depends only on the set of alignments that share its read name, and
 // the insert-size statistics are sums over names, so the work partitions by read name:
 //   k_fx_refs / k_fx_ref_bytes  every GPU's distinct RNAME strings go to the host, which numbers them by string (exact, no hash
@@ -1848,8 +1640,9 @@ __global__ void __launch_bounds__(256) k_fx_home(const FxRec* __restrict__ recs,
 
 unsigned fx_blocks(uint64_t n, unsigned per) { return (unsigned)((n + per - 1) / per); }
 
-// One context of pp_filter_files_multi: its byte ranges as a source, the names it owns as an owner.
-struct FxSide {
+// One context of pp_filter_files_device: its text (the whole files, or one byte range of each) and, over several contexts, the
+// records and names it sends as a source and the names it owns as an owner.
+struct FilterSide {
     pp_ctx* ctx = nullptr;
     TokState* T = nullptr;
     TokFilterBufs* B = nullptr;
@@ -1883,17 +1676,16 @@ struct FxSide {
     uint32_t hist[512];
     uint64_t out_n = 0;
     uint32_t launches = 0;
-    uint64_t text_bytes[2] = {0, 0};
     float h2d_ms = 0;
     pp_tok_stats tst[2];
 };
 
 }  // namespace
 
-// fn(side, g) on every context, each on its own host thread; the first error (its message moved to ctxs[0]) before PP_TOK_HOST,
-// before PP_TOK_NEED8.
+// fn(side, g) on every context, each on its own host thread but the first, which runs on the calling thread; the first error (its
+// message moved to ctxs[0]) before PP_TOK_HOST, before PP_TOK_NEED8.
 template <class F>
-static int fx_all(std::vector<FxSide>& S, F&& fn) {
+static int fx_all(std::vector<FilterSide>& S, F&& fn) {
     std::vector<int> rc(S.size(), PP_OK);
     auto run = [&](size_t g) {
         pp_ctx* ctx = S[g].ctx;
@@ -1918,86 +1710,139 @@ static int fx_copy(pp_ctx* ctx, pp_ctx* dctx, void* dst, const void* src, size_t
     return PP_OK;
 }
 
-int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
-                                 const pp_filter_params* prm, const uint64_t* const cuts[2], pp_filter_result* res, pp_filter_file_stats* fs,
-                                 pp_fused_polish* fuse) {
-    const uint32_t n = (uint32_t)n_ctx;
-    pp_ctx* c0 = ctxs[0];
-    const char* ins[2] = {in1, in2};
-    const char* outs[2] = {out1, out2};
-    memset(fs, 0, sizeof *fs);
-    const auto t_begin = std::chrono::steady_clock::now();
-    std::vector<FxSide> S(n);
-    for (uint32_t g = 0; g < n; ++g) {
-        pp_ctx* ctx = ctxs[g];
-        S[g].ctx = ctx;
-        CK(cudaSetDevice(ctx->device));
-        int rc = tok_state(ctx, &S[g].T);
-        if (rc) { if (g) c0->err = ctx->err; return rc; }
-        if (!S[g].T->fbufs) S[g].T->fbufs = new TokFilterBufs();
-        S[g].B = S[g].T->fbufs;
-        for (uint32_t o = 0; o < n; ++o)                                    // NVLink between the GPUs where the box has it
-            if (ctxs[o]->device != ctx->device) {
-                int can = 0;
-                if (cudaDeviceCanAccessPeer(&can, ctx->device, ctxs[o]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[o]->device, 0);
-                cudaGetLastError();                                          // (already enabled is fine)
-            }
+// Text in, on one context: both texts into HBM, the second streaming in while the first is indexed and parsed (ftok_lines; an empty
+// range is skipped), and the aligned counts.  With `cuts` the context reads bytes [cuts[f][g], cuts[f][g + 1]) of file f, else the
+// whole files.  PP_OK, PP_TOK_HOST (a line the quick parse leaves to the host, a size limit) or an error.
+static int fx_text_in(FilterSide& X, int g, const char* const ins[2], const uint64_t* const cuts[2]) {
+    pp_ctx* ctx = X.ctx;
+    TokState* T = X.T;
+    TokFilterBufs& B = *X.B;
+    cudaStream_t s = ctx->stream;
+    CK(B.status.ensure(sizeof(FStatus)));
+    X.d_st = B.status.as<FStatus>();
+    FStatus h_st;
+    h_st.first_bad[0] = h_st.first_bad[1] = ~0ull; h_st.collision = 0; h_st.pad = 0;
+    CK(cudaMemcpyAsync(X.d_st, &h_st, sizeof h_st, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamSynchronize(s));
+    if (cuts) {
+        T->range_off = {cuts[0][g], cuts[1][g]};
+        T->range_len = {cuts[0][g + 1] - cuts[0][g], cuts[1][g + 1] - cuts[1][g]};
     }
+    for (int k = 0; k < 2; ++k) {
+        int r = prefetch_wait(ctx, T, ins[k], false, cuts ? k : -1);
+        if (r != PP_OK) return r;
+        const uint64_t nb = T->pf.n;
+        const uint8_t* text = T->text[T->pf.buf].as<uint8_t>();
+        const bool unterminated = nb > 0 && T->pf.last != '\n';
+        X.h2d_ms += T->pf.ms;
+        if (k == 0 && (r = prefetch_start(ctx, T, ins[1], false, cuts ? 1 : -1)) != PP_OK) return r;
+        FileDev& fd = X.fd[k];
+        memset(&fd, 0, sizeof fd);
+        fd.text = text;
+        if (nb) r = ftok_lines(ctx, T, k, text, nb, unterminated, B.lines[k], B.tmp[k], X.d_st, &fd, &X.launches);
+        if (r != PP_OK) {
+            if (T->pf.active) { if (T->pf.th.joinable()) T->pf.th.join(); T->pf.active = false; }
+            return r;
+        }
+    }
+    for (int k = 0; k < 2; ++k)
+        if (X.fd[k].n_lines) CK(cudaMemcpyAsync(T->h_tot + k, X.fd[k].s_al + X.fd[k].n_lines, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&h_st, X.d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    for (int k = 0; k < 2; ++k) X.n_al[k] = X.fd[k].n_lines ? T->h_tot[k] : 0;
+    if (h_st.first_bad[0] != ~0ull || h_st.first_bad[1] != ~0ull) return PP_TOK_HOST;
+    if (X.n_al[0] >= 0x7FFFFFFFull || X.n_al[1] >= 0x7FFFFFFFull) return PP_TOK_HOST;
+    return PP_OK;
+}
 
-    // ---- every GPU: its two ranges into HBM, lines, quick parse, local interning (as the one-GPU path)
-    int rc = fx_all(S, [&](FxSide& X, int g) -> int {
+// Local interning, on one context: every QNAME and RNAME of its text gets a slot of one table (k_ftok_intern), and every record
+// confirms its slot's string byte by byte (k_ftok_verify, which flags a collision for the caller's next status read).
+static int fx_intern(FilterSide& X) {
+    pp_ctx* ctx = X.ctx;
+    cudaStream_t s = ctx->stream;
+    uint64_t cap = 1024;
+    while (cap < 3 * (X.n_al[0] + X.n_al[1]) + 1024) cap <<= 1;
+    if (cap > (1ull << 31)) return PP_TOK_HOST;
+    TRY_ALLOC(X.B->table.ensure(cap * 16));
+    X.tb.key = X.B->table.as<unsigned long long>(); X.tb.rep = X.tb.key + cap; X.tb.mask = (uint32_t)(cap - 1);
+    CK(cudaMemsetAsync(X.tb.key, 0, cap * 8, s));
+    CK(cudaMemsetAsync(X.tb.rep, 0xFF, cap * 8, s));
+    for (int k = 0; k < 2; ++k)
+        if (X.fd[k].n_lines) k_ftok_intern<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, X.tb, X.d_st);
+    for (int k = 0; k < 2; ++k)
+        if (X.fd[k].n_lines) k_ftok_verify<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[0], X.fd[1], k, X.tb, X.d_st);
+    X.launches += 4;
+    return PP_OK;
+}
+
+// The filter on one context: its mate arrays written straight from its lines (k_ftok_emit), then the whole filter on the device
+// (pp_filter_core: the thresholds are picked there, no host round trips).  With `fuse` the verdicts move out of the context's
+// scratch buffer, which the polish tokeniser uses next.
+template <class Lap>
+static int filter_one(FilterSide& X, const pp_filter_params* prm_in, pp_filter_result* res, bool fuse, Lap&& lap) {
+    pp_ctx* ctx = X.ctx;
+    TokFilterBufs& B = *X.B;
+    cudaStream_t s = ctx->stream;
+    int rc = fx_intern(X);
+    if (rc != PP_OK) return rc;
+    Mate mates[2];
+    for (int k = 0; k < 2; ++k) {
+        const size_t na = (size_t)X.n_al[k];
+        TRY_ALLOC(B.mate[k].ensure(na * 17 + 5 * 256));
+        uint8_t* mb = B.mate[k].as<uint8_t>();
+        auto up = [](size_t v) { return (v + 255) & ~size_t(255); };
+        MateOut mo;
+        mo.name_id = (uint32_t*)mb; mo.contig = (uint32_t*)(mb + up(na * 4)); mo.ref_start = (uint32_t*)(mb + 2 * up(na * 4));
+        mo.ref_end = (uint32_t*)(mb + 3 * up(na * 4)); mo.flags = mb + 4 * up(na * 4);
+        k_ftok_emit<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], mo);
+        mates[k].name_id = mo.name_id; mates[k].contig = mo.contig; mates[k].ref_start = mo.ref_start; mates[k].ref_end = mo.ref_end;
+        mates[k].flags = mo.flags; mates[k].cnt = nullptr; mates[k].head = nullptr; mates[k].next = nullptr; mates[k].pass = nullptr;
+        mates[k].n = (uint32_t)na;
+    }
+    X.launches += 2;
+    FStatus h_st;
+    CK(cudaMemcpyAsync(&h_st, X.d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    if (h_st.collision) return PP_TOK_HOST;
+    lap(1);
+
+    pp_filter_params prm = *prm_in;
+    prm.n_names = X.tb.mask + 1ull;
+    res->pass1 = nullptr; res->pass2 = nullptr;
+    const uint8_t* d_pass[2] = {nullptr, nullptr};
+    uint64_t np[2] = {0, 0};
+    CK(cudaEventRecord(ctx->ev[0], s));
+    rc = pp_filter_core(ctx, mates, &prm, res, d_pass, np);
+    if (rc != PP_OK) return rc;
+    X.launches += res->timing.launches;
+    for (int k = 0; k < 2; ++k) { X.np[k] = np[k]; X.pass[k] = (uint8_t*)d_pass[k]; }
+    if (fuse) {
+        CK(B.passkeep.ensure(X.n_al[0] + X.n_al[1] + 64));
+        uint8_t* keep = B.passkeep.as<uint8_t>();
+        CK(cudaMemcpyAsync(keep, d_pass[0], X.n_al[0], cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync(keep + X.n_al[0], d_pass[1], X.n_al[1], cudaMemcpyDeviceToDevice, s));
+        CK(cudaStreamSynchronize(s));
+        X.pass[0] = keep; X.pass[1] = keep + X.n_al[0];
+    }
+    return PP_OK;
+}
+
+// The filter over several contexts (see the comment above the k_fx_ kernels): the records meet on the context that owns their read
+// name, and the pair counts and the radix select's histograms are summed on the host.  The verdicts end up in every source's pass[k].
+template <class Lap>
+static int filter_exchange(std::vector<FilterSide>& S, const pp_filter_params* prm, pp_filter_result* res, Lap&& lap) {
+    const uint32_t n = (uint32_t)S.size();
+    // ---- every context: local interning, then its distinct RNAMEs with their bytes
+    int rc = fx_all(S, [&](FilterSide& X, int) -> int {
         pp_ctx* ctx = X.ctx;
         TokState* T = X.T;
         TokFilterBufs& B = *X.B;
         cudaStream_t s = ctx->stream;
-        CK(B.status.ensure(sizeof(FStatus)));
-        X.d_st = B.status.as<FStatus>();
-        FStatus h_st;
-        h_st.first_bad[0] = h_st.first_bad[1] = ~0ull; h_st.collision = 0; h_st.pad = 0;
-        CK(cudaMemcpyAsync(X.d_st, &h_st, sizeof h_st, cudaMemcpyHostToDevice, s));
-        CK(cudaStreamSynchronize(s));
-        T->range_off = {cuts[0][g], cuts[1][g]};
-        T->range_len = {cuts[0][g + 1] - cuts[0][g], cuts[1][g + 1] - cuts[1][g]};
-        uint32_t launches = 0;
-        for (int k = 0; k < 2; ++k) {
-            int r = prefetch_wait(ctx, T, ins[k], false, k);
-            if (r != PP_OK) return r;
-            const uint64_t nb = T->pf.n;
-            const uint8_t* text = T->text[T->pf.buf].as<uint8_t>();
-            const bool unterminated = nb > 0 && T->pf.last != '\n';
-            X.h2d_ms += T->pf.ms;
-            X.text_bytes[k] = nb;
-            if (k == 0 && (r = prefetch_start(ctx, T, ins[1], false, 1)) != PP_OK) return r;
-            FileDev& fd = X.fd[k];
-            memset(&fd, 0, sizeof fd);
-            fd.text = text;
-            if (nb) r = ftok_lines(ctx, T, k, text, nb, unterminated, B.lines[k], B.tmp[k], X.d_st, &fd, &launches);
-            if (r != PP_OK) {
-                if (T->pf.active) { if (T->pf.th.joinable()) T->pf.th.join(); T->pf.active = false; }
-                return r;
-            }
-        }
-        for (int k = 0; k < 2; ++k)
-            if (X.fd[k].n_lines) CK(cudaMemcpyAsync(T->h_tot + k, X.fd[k].s_al + X.fd[k].n_lines, 8, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(&h_st, X.d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        CK(cudaGetLastError());
-        for (int k = 0; k < 2; ++k) X.n_al[k] = X.fd[k].n_lines ? T->h_tot[k] : 0;
-        if (h_st.first_bad[0] != ~0ull || h_st.first_bad[1] != ~0ull) return PP_TOK_HOST;
-        if (X.n_al[0] >= 0x7FFFFFFFull || X.n_al[1] >= 0x7FFFFFFFull) return PP_TOK_HOST;
-        uint64_t cap = 1024;
-        while (cap < 3 * (X.n_al[0] + X.n_al[1]) + 1024) cap <<= 1;
-        if (cap > (1ull << 31)) return PP_TOK_HOST;
-        TRY_ALLOC(B.table.ensure(cap * 16));
-        X.tb.key = B.table.as<unsigned long long>(); X.tb.rep = X.tb.key + cap; X.tb.mask = (uint32_t)(cap - 1);
+        int r = fx_intern(X);
+        if (r != PP_OK) return r;
         X.slot_val = (uint32_t*)X.tb.key;                                   // (the keys are done with once the slots are verified)
-        CK(cudaMemsetAsync(X.tb.key, 0, cap * 8, s));
-        CK(cudaMemsetAsync(X.tb.rep, 0xFF, cap * 8, s));
-        for (int k = 0; k < 2; ++k)
-            if (X.fd[k].n_lines) k_ftok_intern<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, X.tb, X.d_st);
-        for (int k = 0; k < 2; ++k)
-            if (X.fd[k].n_lines) k_ftok_verify<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[0], X.fd[1], k, X.tb, X.d_st);
-        // the distinct RNAMEs of this GPU, with their bytes
         uint64_t rcap = std::max<uint64_t>(1024, B.fx_refs.cap / 2 / sizeof(FxRef));
         for (;;) {
             TRY_ALLOC(B.fx_refs.ensure(2 * rcap * sizeof(FxRef) + 64));
@@ -2006,6 +1851,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
             CK(cudaMemsetAsync(d_n, 0, 8, s));
             for (int k = 0; k < 2; ++k)
                 if (X.fd[k].n_lines) k_fx_refs<<<fx_blocks(X.fd[k].n_lines, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(X.fd[k], k, X.tb, d_refs, d_n, rcap);
+            FStatus h_st;
             CK(cudaMemcpyAsync(T->h_tot, d_n, 8, cudaMemcpyDeviceToHost, s));
             CK(cudaMemcpyAsync(&h_st, X.d_st, sizeof h_st, cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
@@ -2032,21 +1878,16 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
             }
             break;
         }
-        X.launches = launches + 6;
+        X.launches += 2;
         return PP_OK;
     });
     if (rc != PP_OK) return rc;
-    uint64_t n_al_total[2] = {0, 0};
-    for (FxSide& X : S) for (int k = 0; k < 2; ++k) { n_al_total[k] += X.n_al[k]; fs->text_bytes[k] += X.text_bytes[k]; }
-    for (int k = 0; k < 2; ++k) fs->alignments[k] = n_al_total[k];
-    if (n_al_total[0] == 0 || n_al_total[1] == 0) return PP_TOK_HOST;    // "no alignments found in ..." is worded by the host path
-    if (n_al_total[0] >= 0x7FFFFFFFull || n_al_total[1] >= 0x7FFFFFFFull) return PP_TOK_HOST;
-    fs->phase_ms[0] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+    lap(0);
 
     // ---- global RNAME ids: numbered by string, in the order the GPUs list them
     {
         std::unordered_map<std::string, uint32_t> global;
-        for (FxSide& X : S) {
+        for (FilterSide& X : S) {
             X.ref_global.resize(X.refs.size());
             for (size_t j = 0; j < X.refs.size(); ++j) {
                 const std::string name((const char*)X.ref_bytes.data() + X.ref_off[j], X.refs[j].len);
@@ -2055,7 +1896,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         }
     }
     // ---- count what goes where
-    rc = fx_all(S, [&](FxSide& X, int) -> int {
+    rc = fx_all(S, [&](FilterSide& X, int) -> int {
         pp_ctx* ctx = X.ctx;
         cudaStream_t s = ctx->stream;
         TokFilterBufs& B = *X.B;
@@ -2089,7 +1930,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         S[d].rx_names = at_names; S[d].rx_bytes = at_bytes; S[d].rx_recs[0] = at_recs[0]; S[d].rx_recs[1] = at_recs[1];
     }
     for (uint32_t g = 0; g < n; ++g) {
-        FxSide& X = S[g];
+        FilterSide& X = S[g];
         X.plan.assign(n, FxPlan{});
         X.st_names = X.st_bytes = X.st_recs[0] = X.st_recs[1] = 0;
         for (uint32_t d = 0; d < n; ++d) {
@@ -2104,7 +1945,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
     auto rec_base = [&](uint32_t g, uint32_t d, int k) { uint64_t b = 0; for (uint32_t h = 0; h < g; ++h) b += S[h].cnt[d].recs[k]; return b; };
 
     // ---- staging (source) and receive buffers (owner); then the pieces travel
-    rc = fx_all(S, [&](FxSide& X, int) -> int {
+    rc = fx_all(S, [&](FilterSide& X, int) -> int {
         pp_ctx* ctx = X.ctx;
         cudaStream_t s = ctx->stream;
         TokFilterBufs& B = *X.B;
@@ -2138,10 +1979,10 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         return PP_OK;
     });
     if (rc != PP_OK) return rc;
-    rc = fx_all(S, [&](FxSide& X, int g) -> int {
+    rc = fx_all(S, [&](FilterSide& X, int g) -> int {
         for (uint32_t dd = 0; dd < n; ++dd) {
             const uint32_t d = ((uint32_t)g + dd) % n;                      // (the sources start on different destinations)
-            FxSide& D = S[d];
+            FilterSide& D = S[d];
             const FxPlan& p = X.plan[d];
             const FxCount& c = X.cnt[d];
             int r = fx_copy(X.ctx, D.ctx, D.r_names + p.name_base, X.s_names + p.stage_name, c.names * sizeof(FxName));
@@ -2155,10 +1996,10 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         return PP_OK;
     });
     if (rc != PP_OK) return rc;
-    fs->phase_ms[1] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count() - fs->phase_ms[0];
+    lap(1);
 
     // ---- owners: intern and verify the names they received, their two Mate arrays, unique pairs
-    rc = fx_all(S, [&](FxSide& X, int) -> int {
+    rc = fx_all(S, [&](FilterSide& X, int) -> int {
         pp_ctx* ctx = X.ctx;
         cudaStream_t s = ctx->stream;
         TokFilterBufs& B = *X.B;
@@ -2206,11 +2047,11 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
 
     // ---- orientation from the summed pair counts, thresholds by a radix select over all owners (filter.rs:148-186)
     unsigned long long pairs[4] = {0, 0, 0, 0};
-    for (FxSide& X : S) for (int i = 0; i < 4; ++i) pairs[i] += X.pairs[i];
+    for (FilterSide& X : S) for (int i = 0; i < 4; ++i) pairs[i] += X.pairs[i];
     for (int i = 0; i < 4; ++i) res->pairs[i] = pairs[i];
     int chosen = 0;
     unsigned long long n_sizes = 0;
-    rc = filter_orientation(c0, prm, pairs, &chosen, &n_sizes);
+    rc = filter_orientation(S[0].ctx, prm, pairs, &chosen, &n_sizes);
     if (rc != PP_OK) return rc;
     res->orientation = chosen;
     bool in_range[2];
@@ -2218,10 +2059,10 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
     filter_ranks(prm, n_sizes, rank, in_range);
     uint32_t prefix[2] = {0, 0}, done_mask = 0;
     for (const int shift : FILTER_SHIFTS) {
-        rc = fx_all(S, [&](FxSide& X, int) { return filter_hist(X.ctx, X.f, (uint32_t)chosen, shift, done_mask, prefix, X.hist, &X.launches); });
+        rc = fx_all(S, [&](FilterSide& X, int) { return filter_hist(X.ctx, X.f, (uint32_t)chosen, shift, done_mask, prefix, X.hist, &X.launches); });
         if (rc != PP_OK) return rc;
         uint32_t hist[512] = {};
-        for (FxSide& X : S) for (int i = 0; i < 512; ++i) hist[i] += X.hist[i];
+        for (FilterSide& X : S) for (int i = 0; i < 512; ++i) hist[i] += X.hist[i];
         for (int r = 0; r < 2; ++r) prefix[r] |= filter_pick_digit(hist + r * 256, rank[r]) << shift;
         done_mask |= 255u << shift;
     }
@@ -2229,7 +2070,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
     res->high = in_range[1] ? prefix[1] : 0;
 
     // ---- verdicts on the owners, then home to the sources
-    rc = fx_all(S, [&](FxSide& X, int) -> int {
+    rc = fx_all(S, [&](FilterSide& X, int) -> int {
         pp_ctx* ctx = X.ctx;
         cudaStream_t s = ctx->stream;
         filter_pass(ctx, X.f, res->low, res->high, (uint32_t)chosen, &X.launches);
@@ -2239,10 +2080,10 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         return PP_OK;
     });
     if (rc != PP_OK) return rc;
-    rc = fx_all(S, [&](FxSide& D, int d) -> int {
+    rc = fx_all(S, [&](FilterSide& D, int d) -> int {
         for (uint32_t gg = 0; gg < n; ++gg) {
             const uint32_t g = ((uint32_t)d + gg) % n;
-            FxSide& X = S[g];
+            FilterSide& X = S[g];
             for (int k = 0; k < 2; ++k) {
                 const int r = fx_copy(D.ctx, X.ctx, X.ret + X.plan[(uint32_t)d].stage_rec[k], D.f.m[k].pass + rec_base(g, (uint32_t)d, k),
                                       X.cnt[(uint32_t)d].recs[k]);
@@ -2254,7 +2095,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         return PP_OK;
     });
     if (rc != PP_OK) return rc;
-    rc = fx_all(S, [&](FxSide& X, int) -> int {
+    return fx_all(S, [&](FilterSide& X, int) -> int {
         pp_ctx* ctx = X.ctx;
         const uint64_t st_recs = X.st_recs[0] + X.st_recs[1];
         if (st_recs) { k_fx_home<<<fx_blocks(st_recs, 256), 256, 0, ctx->stream>>>(X.s_recs, st_recs, X.ret, X.pass[0], X.pass[1]); X.launches++; }
@@ -2262,27 +2103,117 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         CK(cudaGetLastError());
         return PP_OK;
     });
+}
+
+// Writes one output file from its pieces, S[g].out_n bytes in context g's B->out, one after the other.  A regular file gets its final
+// size up front and every piece is written at its offset, in parallel (a shared mapping or pwrite(); one thread per piece after the
+// first).  Anything else - a FIFO, >(gzip ...), /dev/stdout into a pipe, /dev/null - cannot be truncated or written at offsets: the
+// pieces are streamed in order with write(), like the reference's BufWriter (filter.rs:296-349).  Errors are reported on S[0]'s context.
+static int write_pieces(const std::vector<FilterSide>& S, const char* path, uint64_t* out_bytes) {
+    pp_ctx* c0 = S[0].ctx;
+    const size_t n = S.size();
+    std::vector<uint64_t> base(n + 1, 0);
+    for (size_t g = 0; g < n; ++g) base[g + 1] = base[g] + S[g].out_n;
+    const uint64_t out_n = base[n];
+    struct stat osb;
+    const bool special = stat(path, &osb) == 0 && !S_ISREG(osb.st_mode);
+    const int ofd = special ? open(path, O_WRONLY) : open(path, O_RDWR | O_CREAT | O_TRUNC, 0666);
+    if (ofd < 0) return c0->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + path + "\"");
+    std::vector<int> wrc(n, PP_OK), cuda_err(n, 0);
+    bool stream_out = special;
+    if (out_n && !stream_out && ftruncate(ofd, (off_t)out_n) != 0) stream_out = true;
+    if (out_n && stream_out) {
+        for (size_t g = 0; g < n && wrc[0] == PP_OK; ++g)
+            if (S[g].out_n) wrc[0] = download_stream(S[g].ctx->device, S[g].T, S[g].B->out.as<uint8_t>(), ofd, S[g].out_n, &cuda_err[0]);
+    } else if (out_n) {
+        // Stores into a mapping cannot report "no space left" (they raise SIGBUS), so the mapping is only used when the file system has
+        // room to spare; otherwise pwrite() reports the error like the reference does (filter.rs:307-311).
+        struct statvfs vfs;
+        const bool roomy = fstatvfs(ofd, &vfs) == 0 && (uint64_t)vfs.f_bavail * (uint64_t)vfs.f_frsize > 2 * out_n + (64ull << 20);
+        void* map = roomy ? mmap(nullptr, (size_t)out_n, PROT_READ | PROT_WRITE, MAP_SHARED, ofd, 0) : MAP_FAILED;
+        if (map == MAP_FAILED) map = nullptr;
+        auto put = [&](size_t g) {
+            wrc[g] = download_file(S[g].ctx->device, S[g].T, S[g].B->out.as<uint8_t>(), ofd, (uint8_t*)map, S[g].out_n, &cuda_err[g], base[g]);
+        };
+        std::vector<std::thread> th;
+        for (size_t g = 1; g < n; ++g)
+            if (S[g].out_n) th.emplace_back(put, g);
+        if (S[0].out_n) put(0);
+        for (auto& t : th) t.join();
+        if (map && munmap(map, (size_t)out_n) != 0 && wrc[0] == PP_OK) wrc[0] = PP_ERR_IO;
+    }
+    int w = PP_OK, ce = 0;
+    for (size_t g = 0; g < n; ++g) if (wrc[g] != PP_OK && w == PP_OK) { w = wrc[g]; ce = cuda_err[g]; }
+    if (close(ofd) != 0 && w == PP_OK) w = PP_ERR_IO;
+    if (w == PP_ERR_IO) return c0->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + path + "\"");
+    if (w == PP_ERR_CUDA) return c0->fail_cuda((cudaError_t)ce, "filtered SAM download", __FILE__, __LINE__);
+    *out_bytes = out_n;
+    return PP_OK;
+}
+
+int pp_filter_files_device(pp_ctx* const* ctxs, int n_ctx, const char* in1, const char* in2, const char* out1, const char* out2,
+                           const pp_filter_params* prm, const uint64_t* const cuts[2], pp_filter_result* res, pp_filter_file_stats* fs,
+                           pp_fused_polish* fuse) {
+    const uint32_t n = (uint32_t)n_ctx;
+    pp_ctx* c0 = ctxs[0];
+    const char* ins[2] = {in1, in2};
+    const char* outs[2] = {out1, out2};
+    memset(fs, 0, sizeof *fs);
+    const auto t_begin = std::chrono::steady_clock::now();
+    auto t_mark = t_begin;
+    auto lap = [&](int i) { const auto now = std::chrono::steady_clock::now(); fs->phase_ms[i] += std::chrono::duration<float, std::milli>(now - t_mark).count(); t_mark = now; };
+    std::vector<FilterSide> S(n);
+    for (uint32_t g = 0; g < n; ++g) {
+        pp_ctx* ctx = ctxs[g];
+        S[g].ctx = ctx;
+        CK(cudaSetDevice(ctx->device));
+        int rc = tok_state(ctx, &S[g].T);
+        if (rc) { if (g) c0->err = ctx->err; return rc; }
+        if (!S[g].T->fbufs) S[g].T->fbufs = new TokFilterBufs();
+        S[g].B = S[g].T->fbufs;
+        for (uint32_t o = 0; o < n; ++o)                                    // NVLink between the GPUs where the box has it
+            if (ctxs[o]->device != ctx->device) {
+                int can = 0;
+                if (cudaDeviceCanAccessPeer(&can, ctx->device, ctxs[o]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[o]->device, 0);
+                cudaGetLastError();                                          // (already enabled is fine)
+            }
+    }
+
+    // ---- every context: its two texts into HBM, lines, quick parse
+    int rc = fx_all(S, [&](FilterSide& X, int g) { return fx_text_in(X, g, ins, cuts); });
+    if (rc != PP_OK) return rc;
+    uint64_t n_al[2] = {0, 0};
+    for (FilterSide& X : S) for (int k = 0; k < 2; ++k) { n_al[k] += X.n_al[k]; fs->text_bytes[k] += X.fd[k].n; }
+    for (int k = 0; k < 2; ++k) fs->alignments[k] = n_al[k];
+    if (n_al[0] == 0 || n_al[1] == 0) return PP_TOK_HOST;               // "no alignments found in ..." is worded by the host path
+    if (n_al[0] >= 0x7FFFFFFFull || n_al[1] >= 0x7FFFFFFFull) return PP_TOK_HOST;
+
+    // ---- the filter: one context on its own, several across the contexts by read name
+    if (n == 1) {
+        lap(0);                                                          // (over several contexts phase 0 also takes the local interning)
+        rc = filter_one(S[0], prm, res, fuse != nullptr, lap);
+    } else {
+        rc = filter_exchange(S, prm, res, lap);
+    }
     if (rc != PP_OK) return rc;
     uint64_t np[2] = {0, 0};
-    for (FxSide& X : S) { np[0] += X.np[0]; np[1] += X.np[1]; }
+    for (FilterSide& X : S) { np[0] += X.np[0]; np[1] += X.np[1]; }
     res->n_pass = np[0] + np[1];
-    for (int k = 0; k < 2; ++k) { fs->pass[k] = np[k]; fs->fail[k] = n_al_total[k] - np[k]; }
-    fs->phase_ms[2] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count() - fs->phase_ms[0] - fs->phase_ms[1];
+    for (int k = 0; k < 2; ++k) { fs->pass[k] = np[k]; fs->fail[k] = n_al[k] - np[k]; }
+    lap(2);
 
-    // ---- output text: every GPU assembles its piece; the pieces go to their offsets (a regular file) or in range order (anything else)
-    float d2h_ms = 0;
+    // ---- output text, file by file: every context assembles its piece (lengths -> offsets -> bytes), one writer puts the pieces in the file
     for (int k = 0; k < 2; ++k) {
         if (!outs[k]) continue;
-        const auto t_out = std::chrono::steady_clock::now();
-        rc = fx_all(S, [&](FxSide& X, int) -> int {
+        rc = fx_all(S, [&](FilterSide& X, int g) -> int {
             pp_ctx* ctx = X.ctx;
             TokState* T = X.T;
             TokFilterBufs& B = *X.B;
             cudaStream_t s = ctx->stream;
             const FileDev& fd = X.fd[k];
-            X.out_n = 0;
-            if (!fd.n_lines) return PP_OK;
             const uint64_t nl = fd.n_lines;
+            X.out_n = 0;
+            if (!nl) return PP_OK;
             CK(B.table.ensure((nl + 2) * 8));                                // the local intern table is done with: reuse it
             unsigned long long* out_off = B.table.as<unsigned long long>();
             k_ftok_outlen<<<fx_blocks(nl + 1, TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(fd, X.pass[k], out_off);
@@ -2294,69 +2225,44 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
             CK(cudaMemcpyAsync(T->h_tot, out_off + nl, 8, cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
             X.out_n = T->h_tot[0];
-            CK(B.out.ensure(X.out_n + 64));
+            if (g == 0) lap(3);                                              // (context 0 runs on the calling thread)
+            TRY_ALLOC(B.out.ensure(X.out_n + 64));
             k_ftok_copy<<<fx_blocks(nl * 32, 256), 256, 0, s>>>(fd, X.pass[k], out_off, B.out.as<uint8_t>());
             CK(cudaStreamSynchronize(s));
             CK(cudaGetLastError());
-            X.launches += 3;
+            X.launches += n == 1 ? 4 : 3;                                    // (the N-context count takes the scan as one launch)
+            if (g == 0) lap(4);
             return PP_OK;
         });
         if (rc != PP_OK) return rc;
-        std::vector<uint64_t> base(n + 1, 0);
-        for (uint32_t g = 0; g < n; ++g) base[g + 1] = base[g] + S[g].out_n;
-        const uint64_t out_n = base[n];
-        struct stat osb;
-        const bool special = stat(outs[k], &osb) == 0 && !S_ISREG(osb.st_mode);
-        const int ofd = special ? open(outs[k], O_WRONLY) : open(outs[k], O_RDWR | O_CREAT | O_TRUNC, 0666);
-        if (ofd < 0) return c0->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + outs[k] + "\"");
-        std::vector<int> wrc(n, PP_OK), cuda_err(n, 0);
-        bool stream_out = special;
-        if (out_n && !stream_out && ftruncate(ofd, (off_t)out_n) != 0) stream_out = true;
-        if (out_n && stream_out) {
-            for (uint32_t g = 0; g < n && wrc[0] == PP_OK; ++g)
-                if (S[g].out_n) wrc[0] = download_stream(S[g].ctx->device, S[g].T, S[g].B->out.as<uint8_t>(), ofd, S[g].out_n, &cuda_err[0]);
-        } else if (out_n) {
-            // (the one-GPU rule: a mapping only where the file system has room to spare, else pwrite() reports a full disk)
-            struct statvfs vfs;
-            const bool roomy = fstatvfs(ofd, &vfs) == 0 && (uint64_t)vfs.f_bavail * (uint64_t)vfs.f_frsize > 2 * out_n + (64ull << 20);
-            void* map = roomy ? mmap(nullptr, (size_t)out_n, PROT_READ | PROT_WRITE, MAP_SHARED, ofd, 0) : MAP_FAILED;
-            if (map == MAP_FAILED) map = nullptr;
-            std::vector<std::thread> th;
-            for (uint32_t g = 0; g < n; ++g)
-                if (S[g].out_n)
-                    th.emplace_back([&, g] { wrc[g] = download_file(S[g].ctx->device, S[g].T, S[g].B->out.as<uint8_t>(), ofd, (uint8_t*)map, S[g].out_n,
-                                                                    &cuda_err[g], base[g]); });
-            for (auto& t : th) t.join();
-            if (map && munmap(map, (size_t)out_n) != 0 && wrc[0] == PP_OK) wrc[0] = PP_ERR_IO;
-        }
-        int w = PP_OK, ce = 0;
-        for (uint32_t g = 0; g < n; ++g) if (wrc[g] != PP_OK && w == PP_OK) { w = wrc[g]; ce = cuda_err[g]; }
-        if (close(ofd) != 0 && w == PP_OK) w = PP_ERR_IO;
-        d2h_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_out).count();
-        if (w == PP_ERR_IO) return c0->fail(PP_ERR_IO, std::string("unable to write alignments to \"") + outs[k] + "\"");
-        if (w == PP_ERR_CUDA) return c0->fail_cuda((cudaError_t)ce, "filtered SAM download", __FILE__, __LINE__);
-        fs->out_bytes[k] = out_n;
+        const auto t0 = std::chrono::steady_clock::now();
+        rc = write_pieces(S, outs[k], &fs->out_bytes[k]);
+        fs->d2h_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        if (rc != PP_OK) return rc;
+        lap(5);
     }
-    fs->d2h_ms = d2h_ms;
-    for (FxSide& X : S) { fs->launches += X.launches; fs->h2d_ms = std::max(fs->h2d_ms, X.h2d_ms); }
+    for (FilterSide& X : S) { fs->launches += X.launches; fs->h2d_ms = std::max(fs->h2d_ms, X.h2d_ms); }
 
-    // ---- filter-polish: every GPU tokenises its ranges for polish, the verdicts become ZP flags; pp_tok_exchange_finish comes next
+    // ---- filter-polish: every context tokenises its text for polish (pp_tok_*), with its verdicts as ZP flags; byte ranges get the
+    // range marks and the empty-range rule of pp_tok_add_files
     if (fuse) {
         fuse->rc = PP_TOK_HOST;
         for (int bits = 4;; bits = 8) {
-            rc = fx_all(S, [&](FxSide& X, int g) -> int {
+            rc = fx_all(S, [&](FilterSide& X, int g) -> int {
                 pp_ctx* ctx = X.ctx;
                 TokState* T = X.T;
                 int r = pp_tok_begin(ctx, fuse->fasta, fuse->careful, bits);
-                const uint64_t off[2] = {cuts[0][g], cuts[1][g]}, len[2] = {cuts[0][g + 1] - cuts[0][g], cuts[1][g + 1] - cuts[1][g]};
-                if (r == PP_OK) r = pp_tok_set_ranges(ctx, off, len, 2);
+                if (r == PP_OK && cuts) {
+                    const uint64_t off[2] = {cuts[0][g], cuts[1][g]}, len[2] = {cuts[0][g + 1] - cuts[0][g], cuts[1][g + 1] - cuts[1][g]};
+                    r = pp_tok_set_ranges(ctx, off, len, 2);
+                }
                 if (r != PP_OK) return r;
-                T->expect_total = len[0] + len[1];
+                T->expect_total = X.fd[0].n + X.fd[1].n;
                 memset(X.tst, 0, sizeof X.tst);
                 for (int k = 0; k < 2; ++k) {
-                    T->marks.push_back({T->aln_base, T->ops_base, T->blk_base, T->read_base});
+                    if (cuts) T->marks.push_back({T->aln_base, T->ops_base, T->blk_base, T->read_base});
                     const uint64_t a0 = T->aln_base;
-                    r = tok_process(ctx, T, X.fd[k].text, X.fd[k].n, X.fd[k].unterminated != 0, &X.tst[k], true);
+                    r = tok_process(ctx, T, X.fd[k].text, X.fd[k].n, X.fd[k].unterminated != 0, &X.tst[k], cuts != nullptr);
                     if (r == PP_OK && X.tst[k].alignments != X.n_al[k]) r = PP_TOK_HOST;       // (cannot happen: same lines, same rule)
                     if (r != PP_OK) { T->active = false; return r; }
                     if (X.n_al[k]) {
@@ -2365,7 +2271,7 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
                         CK(cudaGetLastError());
                     }
                 }
-                T->marks.push_back({T->aln_base, T->ops_base, T->blk_base, T->read_base});
+                if (cuts) T->marks.push_back({T->aln_base, T->ops_base, T->blk_base, T->read_base});
                 return PP_OK;
             });
             if (rc == PP_TOK_NEED8 && bits == 4) continue;
@@ -2375,11 +2281,11 @@ int pp_filter_files_device_multi(pp_ctx* const* ctxs, int n_ctx, const char* in1
         if (rc < 0) return rc;
         if (rc == PP_OK) {
             memset(fuse->stats, 0, sizeof fuse->stats);
-            for (FxSide& X : S)
+            for (FilterSide& X : S)
                 for (int k = 0; k < 2; ++k) {
                     fuse->stats[k].alignments += X.tst[k].alignments; fuse->stats[k].reads += X.tst[k].reads; fuse->stats[k].lines += X.tst[k].lines;
                 }
-            fuse->n_aln = n_al_total[0] + n_al_total[1];
+            fuse->n_aln = n_al[0] + n_al[1];
         }
         fuse->rc = rc;
     }
