@@ -285,17 +285,20 @@ def model_quick(line):
     return (1, start & 0xFFFFFFFF, end, 1 if flag & 16 else 0)
 
 
-def ftok_cpu(H, text):
+def ftok_cpu(H, text, ref_hash=False):
+    """The quick parse's columns per line; with ref_hash, the RNAME keys follow as a ninth array."""
     nl = text.count(b"\n") + 2
     kind = np.zeros(nl, np.uint8); rs = np.zeros(nl, np.uint32); re_ = np.zeros(nl, np.uint32); rev = np.zeros(nl, np.uint8)
     nlen = np.zeros(nl, np.uint32); rrel = np.zeros(nl, np.uint32); rlen = np.zeros(nl, np.uint32); nh = np.zeros(nl, np.uint64)
+    rh = np.zeros(nl, np.uint64)
     n_out = C.c_uint64()
     H.ftok_cpu.restype = C.c_int
-    rc = H.ftok_cpu(C.c_char_p(text), C.c_uint64(len(text)), C.c_uint64(nl), *[a.ctypes.data_as(C.c_void_p) for a in (kind, rs, re_, rev, nlen, rrel, rlen, nh)],
-                    C.byref(n_out))
+    rc = H.ftok_cpu(C.c_char_p(text), C.c_uint64(len(text)), C.c_uint64(nl),
+                    *[a.ctypes.data_as(C.c_void_p) for a in (kind, rs, re_, rev, nlen, rrel, rlen, nh, rh)], C.byref(n_out))
     assert rc == 0
     n = n_out.value
-    return kind[:n], rs[:n], re_[:n], rev[:n], nlen[:n], rrel[:n], rlen[:n], nh[:n]
+    out = (kind[:n], rs[:n], re_[:n], rev[:n], nlen[:n], rrel[:n], rlen[:n], nh[:n])
+    return out + (rh[:n],) if ref_hash else out
 
 
 def split_lines(text):

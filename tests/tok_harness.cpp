@@ -99,7 +99,7 @@ extern "C" int tok_cpu(const char* text_in, uint64_t n, const char* const* names
 
 // The quick parse of `polypolish filter` (tok_line.h parse_line_quick), line by line.
 extern "C" int ftok_cpu(const char* text_in, uint64_t n, uint64_t cap_lines, uint8_t* kind, uint32_t* ref_start, uint32_t* ref_end, uint8_t* rev,
-                        uint32_t* name_len, uint32_t* ref_rel, uint32_t* ref_len, uint64_t* name_hash, uint64_t* n_lines_out) {
+                        uint32_t* name_len, uint32_t* ref_rel, uint32_t* ref_len, uint64_t* name_hash, uint64_t* ref_hash, uint64_t* n_lines_out) {
     std::vector<uint64_t> buf((n + 15) / 8 + 8, 0);
     uint8_t* text = reinterpret_cast<uint8_t*>(buf.data());
     memcpy(text, text_in, n);
@@ -117,10 +117,13 @@ extern "C" int ftok_cpu(const char* text_in, uint64_t n, uint64_t cap_lines, uin
         tok::FLineRec r;
         kind[i] = tok::parse_line_quick(x, s, e, r);
         ref_start[i] = r.ref_start; ref_end[i] = r.ref_end; rev[i] = r.rev; name_len[i] = r.name_len; ref_rel[i] = r.ref_rel; ref_len[i] = r.ref_len;
-        name_hash[i] = r.name_hash;
+        name_hash[i] = r.name_hash; ref_hash[i] = r.ref_hash;
     }
     return 0;
 }
+
+// The contig table's key of a name (tok_table.h).
+extern "C" uint64_t fnv1a_cpu(const char* s, uint64_t n) { return tok::fnv1a(std::string(s, (size_t)n)); }
 
 // The upload-side QUAL stripping (tok_strip.h).
 #include "../polypolish_b200/csrc/tok_strip.h"
