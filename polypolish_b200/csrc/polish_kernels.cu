@@ -130,12 +130,10 @@ static void fill_data(pp_ctx* ctx, DevData& d) {
     const uint64_t G = ctx->G;
     memset(&d, 0, sizeof d);
     d.n_aln = ctx->n_aln;
-    d.contig = ctx->b[B_CONTIG].as<uint32_t>(); d.ref_start = ctx->b[B_REFSTART].as<uint32_t>();
-    d.read_id = ctx->b[B_READID].as<uint32_t>(); d.seq_off = ctx->b[B_SEQOFF].as<uint32_t>();
-    d.cigar_off = ctx->b[B_CIGOFF].as<uint32_t>(); d.nm = ctx->b[B_NM].as<uint32_t>();
-    d.cigar_ops = ctx->b[B_CIGOPS].as<uint32_t>(); d.seq_len = ctx->b[B_SEQLEN].as<uint16_t>();
-    d.n_cigar = ctx->b[B_NCIG].as<uint16_t>(); d.flags = ctx->b[B_FLAGS].as<uint8_t>();
-    d.seq_pool = ctx->b[B_SEQPOOL].as<uint8_t>(); d.draft = ctx->b[B_DRAFT].as<uint8_t>();
+    const DsArrays a = ds_view(ctx->b + B_CONTIG);
+    d.contig = a.contig; d.ref_start = a.ref_start; d.read_id = a.read_id; d.seq_off = a.seq_off; d.cigar_off = a.cigar_off; d.nm = a.nm;
+    d.cigar_ops = a.cigar_ops; d.seq_len = a.seq_len; d.n_cigar = a.n_cigar; d.flags = a.flags; d.seq_pool = a.seq_pool;
+    d.draft = ctx->b[B_DRAFT].as<uint8_t>();
     d.contig_off = ctx->b[B_CTGOFF].as<unsigned long long>(); d.n_contigs = ctx->n_contigs; d.G = (uint32_t)G;
     d.n_bins = (uint32_t)((G + PP_BIN - 1) >> PP_BIN_SHIFT); d.n_tiles = (uint32_t)((G + TL_T - 1) / TL_T);
     d.recs = ctx->b[B_RECS].as<TileRec>(); d.key = ctx->b[B_KEY].as<uint32_t>(); d.val = ctx->b[B_VAL].as<uint32_t>();
@@ -306,18 +304,15 @@ extern "C" int pp_dataset_upload(pp_ctx* ctx, const pp_contigs* c, const pp_alig
     CK(cudaSetDevice(ctx->device));
     ctx->have_ds = false;
     int rc;
-    if ((rc = upload(ctx, B_CONTIG, a->contig, a->n_aln))) return rc;
-    if ((rc = upload(ctx, B_REFSTART, a->ref_start, a->n_aln))) return rc;
-    if (a->read_id) { if ((rc = upload(ctx, B_READID, a->read_id, a->n_aln))) return rc; }
-    else CK(ctx->b[B_READID].ensure((size_t)a->n_aln * 4 + 64));
-    if ((rc = upload(ctx, B_SEQOFF, a->seq_off, a->n_aln))) return rc;
-    if ((rc = upload(ctx, B_SEQLEN, a->seq_len, a->n_aln))) return rc;
-    if (a->cigar_off) { if ((rc = upload(ctx, B_CIGOFF, a->cigar_off, a->n_aln))) return rc; }
-    else CK(ctx->b[B_CIGOFF].ensure((size_t)a->n_aln * 4 + 64));
-    if ((rc = upload(ctx, B_NCIG, a->n_cigar, a->n_aln))) return rc;
-    if ((rc = upload(ctx, B_NM, a->nm, a->n_aln))) return rc;
-    if ((rc = upload(ctx, B_FLAGS, a->flags, a->n_aln))) return rc;
-    if ((rc = upload(ctx, B_CIGOPS, a->cigar_ops, a->n_cigar_ops))) return rc;
+    const void* host[DS_N];
+    ds_host(a, host);
+    const uint64_t cnt[3] = {a->n_aln, a->n_cigar_ops, 0};
+    for (int k = 0; k < DS_SEQPOOL; ++k) {                                          // (the sequence pool follows below)
+        const size_t bytes = ds_bytes(k, cnt, 0);
+        CK(ctx->b[B_CONTIG + k].ensure(bytes + 64));
+        const bool derived = !host[k] && (B_CONTIG + k == B_READID || B_CONTIG + k == B_CIGOFF);   // (rebuilt on the device below)
+        if (bytes && !derived) CK(cudaMemcpyAsync(ctx->b[B_CONTIG + k].p, host[k], bytes, cudaMemcpyHostToDevice, ctx->stream));
+    }
     if (a->n_aln && (!a->cigar_off || !a->read_id)) {
         const uint32_t grid = (uint32_t)std::min<uint64_t>((a->n_aln + 255) / 256, (uint64_t)ctx->sm_count * 32);
         uint32_t* co = a->cigar_off ? nullptr : ctx->b[B_CIGOFF].as<uint32_t>();

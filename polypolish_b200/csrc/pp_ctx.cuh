@@ -35,6 +35,52 @@ enum { B_CONTIG, B_REFSTART, B_READID, B_SEQOFF, B_SEQLEN, B_CIGOFF, B_NCIG, B_N
        B_DEPSTART, B_DEPRUN,
        B_TOKLINE, B_TOKTMP, B_TOKNAMES, B_COUNT };
 
+// The resident dataset: DS_N arrays, array k in b[B_CONTIG + k].  Each is sized by one count - records, CIGAR ops or sequence blocks -
+// times its element width; the sequence pool's width is the block bytes of the dataset's seq_bits.
+enum DsCount { DS_RECS, DS_OPS, DS_BLKS };
+struct DsArray { uint32_t width; DsCount count; };          // width 0: the sequence pool
+enum { DS_SEQPOOL = B_SEQPOOL - B_CONTIG, DS_N };
+constexpr DsArray DS_ARRAYS[DS_N] = {
+    {4, DS_RECS},   // B_CONTIG    contig
+    {4, DS_RECS},   // B_REFSTART  ref_start
+    {4, DS_RECS},   // B_READID    read_id
+    {4, DS_RECS},   // B_SEQOFF    seq_off
+    {2, DS_RECS},   // B_SEQLEN    seq_len
+    {4, DS_RECS},   // B_CIGOFF    cigar_off
+    {2, DS_RECS},   // B_NCIG      n_cigar
+    {4, DS_RECS},   // B_NM        nm
+    {1, DS_RECS},   // B_FLAGS     flags
+    {4, DS_OPS},    // B_CIGOPS    cigar_ops
+    {0, DS_BLKS},   // B_SEQPOOL   seq_pool
+};
+__host__ __device__ constexpr uint32_t ds_block_bytes(uint32_t seq_bits) { return seq_bits == 8 ? 32 : 16; }
+inline size_t ds_width(int k, uint32_t seq_bits) { return DS_ARRAYS[k].width ? DS_ARRAYS[k].width : ds_block_bytes(seq_bits); }
+// bytes of array k for n[DS_RECS] records, n[DS_OPS] CIGAR ops and n[DS_BLKS] sequence blocks
+inline size_t ds_bytes(int k, const uint64_t n[3], uint32_t seq_bits) { return (size_t)n[DS_ARRAYS[k].count] * ds_width(k, seq_bits); }
+
+// The typed device pointers of one set of the DS_N arrays (a context's dataset, or a copy of its layout).
+struct DsArrays {
+    uint32_t *contig, *ref_start, *read_id, *seq_off;
+    uint16_t* seq_len;
+    uint32_t* cigar_off;
+    uint16_t* n_cigar;
+    uint32_t* nm;
+    uint8_t* flags;
+    uint32_t* cigar_ops;
+    uint8_t* seq_pool;
+};
+inline DsArrays ds_view(const DevBuf* b) {                  // b[0 .. DS_N - 1] in the order above: ctx->b + B_CONTIG, or a copy's
+    return {b[0].as<uint32_t>(), b[1].as<uint32_t>(), b[2].as<uint32_t>(), b[3].as<uint32_t>(), b[4].as<uint16_t>(), b[5].as<uint32_t>(),
+            b[6].as<uint16_t>(), b[7].as<uint32_t>(), b[8].as<uint8_t>(), b[9].as<uint32_t>(), b[10].as<uint8_t>()};
+}
+
+// The host arrays of `a`, in the order above.
+inline void ds_host(const pp_alignments* a, const void* out[DS_N]) {
+    const void* p[DS_N] = {a->contig, a->ref_start, a->read_id, a->seq_off, a->seq_len, a->cigar_off, a->n_cigar, a->nm, a->flags,
+                           a->cigar_ops, a->seq_pool};
+    for (int k = 0; k < DS_N; ++k) out[k] = p[k];
+}
+
 // A per-position report recorded as runs: whether calls record it (on), whether the last call did (have) and its runs, exactly n
 // long, in b[b_start] (start positions) / b[b_value] (values).
 struct RunReport {

@@ -163,9 +163,7 @@ __global__ void __launch_bounds__(TK_LINE_THREADS) k_tok_parse(ParseArgs a) {
 struct EmitArgs {
     ParseArgs p;
     uint64_t aln_base, ops_base, blk_base;
-    uint32_t *contig, *ref_start, *seq_off, *cigar_off, *nm, *cigar_ops;
-    uint16_t *seq_len, *n_cigar;
-    uint8_t *flags, *seq_pool;
+    DsArrays d;                       // the dataset
     unsigned long long* name_pos;     // [alignments of this file] text offset of the QNAME
     uint32_t* name_len;
 };
@@ -183,19 +181,19 @@ __global__ void __launch_bounds__(TK_LINE_THREADS) k_tok_emit(EmitArgs a) {
     const uint64_t la = a.p.s_al[i], A = a.aln_base + la;
     const uint64_t co = a.ops_base + a.p.s_ops[i], bo = a.blk_base + a.p.s_blk[i];
     const bool star = r.flags & PP_FLAG_SEQSTAR;
-    a.contig[A] = r.contig;
-    a.ref_start[A] = r.ref_start;
-    a.seq_off[A] = star ? 0u : (uint32_t)bo;
-    a.seq_len[A] = (uint16_t)r.slen;
-    a.cigar_off[A] = (uint32_t)co;
-    a.n_cigar[A] = (uint16_t)r.nops;
-    a.nm[A] = r.nm;
-    a.flags[A] = r.flags;
+    a.d.contig[A] = r.contig;
+    a.d.ref_start[A] = r.ref_start;
+    a.d.seq_off[A] = star ? 0u : (uint32_t)bo;
+    a.d.seq_len[A] = (uint16_t)r.slen;
+    a.d.cigar_off[A] = (uint32_t)co;
+    a.d.n_cigar[A] = (uint16_t)r.nops;
+    a.d.nm[A] = r.nm;
+    a.d.flags[A] = r.flags;
     a.name_pos[la] = s;
     a.name_len[la] = r.name_len;
     tok::Txt x(a.p.text);
-    tok::emit_cigar(x, s, r, a.cigar_ops + co);
-    if (tok::emit_seq<BITS>(x, s, r, s_nib, a.seq_pool + bo * (BITS == 4 ? 16 : 32))) a.p.st->need8 = 1;
+    tok::emit_cigar(x, s, r, a.d.cigar_ops + co);
+    if (tok::emit_seq<BITS>(x, s, r, s_nib, a.d.seq_pool + bo * ds_block_bytes(BITS))) a.p.st->need8 = 1;
 }
 
 __global__ void __launch_bounds__(TK_LINE_THREADS) k_tok_heads(const uint8_t* __restrict__ text, uint64_t n_al, const unsigned long long* __restrict__ name_pos,
@@ -330,6 +328,39 @@ static int ensure_keep(pp_ctx* ctx, int which, size_t bytes, size_t keep) {
     return PP_OK;
 }
 
+// The line index of a text on the device (n bytes, zero padded), in two calls.  line_count counts its lines - newlines per 16 KiB tile
+// (k_tok_count), their offsets (a scan, in B_TOKLINE), the total read back - and answers PP_TOK_HOST past the limits; line_starts then
+// writes line_start[0 .. n_lines] into the caller's buffer (k_tok_index).
+struct LineIndex { uint64_t n16, n_tiles, n_lines; const unsigned long long* tile_off; };
+
+static int line_count(pp_ctx* ctx, TokState* T, const uint8_t* text, uint64_t n, bool unterminated, LineIndex* li) {
+    cudaStream_t s = ctx->stream;
+    li->n16 = (n + 15) & ~15ull;
+    li->n_tiles = (li->n16 + TK_TILE - 1) / TK_TILE;
+    li->n_lines = 0;
+    if (li->n_tiles >= 0x7FFFFFFFull) return PP_TOK_HOST;
+    size_t cub_bytes = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int64_t)std::max<uint64_t>(li->n_tiles + 1, 1)));
+    CK(T->cub.ensure(cub_bytes + 256));
+    TRY_ALLOC(ctx->b[B_TOKLINE].ensure((li->n_tiles + 2) * 8));
+    unsigned long long* tile_cnt = ctx->b[B_TOKLINE].as<unsigned long long>();
+    li->tile_off = tile_cnt;
+    if (li->n_tiles) {
+        CK(cudaMemsetAsync(tile_cnt + li->n_tiles, 0, 8, s));
+        k_tok_count<<<(unsigned)li->n_tiles, TK_THREADS, 0, s>>>(text, li->n16, tile_cnt);
+        size_t tb = T->cub.cap;
+        CK(cub::DeviceScan::ExclusiveSum(T->cub.p, tb, tile_cnt, tile_cnt, (int64_t)(li->n_tiles + 1), s));
+        CK(cudaMemcpyAsync(T->h_tot, tile_cnt + li->n_tiles, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        li->n_lines = T->h_tot[0] + (unterminated ? 1 : 0);
+    }
+    return li->n_lines >= 0xFFFFFFF0ull ? PP_TOK_HOST : PP_OK;
+}
+
+static void line_starts(pp_ctx* ctx, const uint8_t* text, const LineIndex& li, unsigned long long* line_start) {
+    k_tok_index<<<(unsigned)li.n_tiles, TK_THREADS, 0, ctx->stream>>>(text, li.n16, li.tile_off, line_start);
+}
+
 int pp_ctx_upload_contigs(pp_ctx* ctx, const pp_contigs* c);
 int pp_ctx_commit_dataset(pp_ctx* ctx, uint64_t n_aln, uint64_t n_reads, uint64_t n_ops, uint64_t seq_bytes, uint32_t seq_bits);
 
@@ -415,28 +446,13 @@ static int tok_process(pp_ctx* ctx, TokState* T, const uint8_t* text, uint64_t n
     uint32_t launches = 0;
     CK(cudaEventRecord(ctx->ev[0], s));
     // ---- lines
-    const uint64_t n16 = (n + 15) & ~15ull;
-    const uint64_t n_tiles = (n16 + TK_TILE - 1) / TK_TILE;
-    if (n_tiles >= 0x7FFFFFFFull) return PP_TOK_HOST;
-    size_t cub_bytes = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int64_t)std::max<uint64_t>(n_tiles + 1, 1)));
-    CK(T->cub.ensure(cub_bytes + 256));
-    TRY_ALLOC(ctx->b[B_TOKLINE].ensure((n_tiles + 2) * 8));
-    unsigned long long* tile_cnt = ctx->b[B_TOKLINE].as<unsigned long long>();
-    uint64_t n_lines = 0;
-    if (n_tiles) {
-        CK(cudaMemsetAsync(tile_cnt + n_tiles, 0, 8, s));
-        k_tok_count<<<(unsigned)n_tiles, TK_THREADS, 0, s>>>(text, n16, tile_cnt);
-        size_t tb = T->cub.cap;
-        CK(cub::DeviceScan::ExclusiveSum(T->cub.p, tb, tile_cnt, tile_cnt, (int64_t)(n_tiles + 1), s));
-        CK(cudaMemcpyAsync(T->h_tot, tile_cnt + n_tiles, 8, cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
-        launches += 3;
-        n_lines = T->h_tot[0] + (unterminated ? 1 : 0);
-    }
+    LineIndex li;
+    int rc = line_count(ctx, T, text, n, unterminated, &li);
+    const uint64_t n_lines = li.n_lines;
     if (stats) stats->lines = n_lines;
+    if (rc != PP_OK) return rc;
+    if (li.n_tiles) launches += 3;
     if (n_lines == 0) return part_of_file ? PP_OK : PP_TOK_HOST;   // "no alignments in <file>": the host packer words it (a byte range may be empty)
-    if (n_lines >= 0xFFFFFFF0ull) return PP_TOK_HOST;
 
     // scratch: line starts | line records | three scan arrays
     size_t off = 0;
@@ -452,9 +468,10 @@ static int tok_process(pp_ctx* ctx, TokState* T, const uint8_t* text, uint64_t n
     pa.st = T->d_st;
     T->h_st->first_bad = ~0ull; T->h_st->need8 = 0; T->h_st->group_err = 0;
     CK(cudaMemcpyAsync(T->d_st, T->h_st, sizeof(TokStatus), cudaMemcpyHostToDevice, s));
-    k_tok_index<<<(unsigned)n_tiles, TK_THREADS, 0, s>>>(text, n16, tile_cnt, (unsigned long long*)(tmp + o_ls));
+    line_starts(ctx, text, li, (unsigned long long*)(tmp + o_ls));
     const unsigned line_grid = (unsigned)((n_lines + 1 + TK_LINE_THREADS - 1) / TK_LINE_THREADS);
     k_tok_parse<<<line_grid, TK_LINE_THREADS, 0, s>>>(pa);
+    size_t cub_bytes = 0;
     CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, pa.s_al, pa.s_al, (int64_t)(n_lines + 1)));
     CK(T->cub.ensure(cub_bytes + 256));
     for (unsigned long long* arr : {pa.s_al, pa.s_ops, pa.s_blk}) {
@@ -475,19 +492,16 @@ static int tok_process(pp_ctx* ctx, TokState* T, const uint8_t* text, uint64_t n
 
     // ---- dataset arrays (kept across files)
     const uint64_t A0 = T->aln_base, A1 = A0 + n_al;
-    const size_t blk_bytes = T->seq_bits == 4 ? 16 : 32;
     // first file of a dataset whose total text size is known: size the arrays for all of it (no regrowth, no cudaFree later)
     double grow = 1.0;
     if (A0 == 0 && T->expect_total > n && n > 0) grow = std::min(64.0, 1.03 * (double)T->expect_total / (double)n);
     auto want = [&](uint64_t items, size_t each) { return (size_t)((double)items * grow) * each; };
-    int rc;
-    for (int w : {B_CONTIG, B_REFSTART, B_READID, B_SEQOFF, B_CIGOFF, B_NM})
-        if ((rc = ensure_keep(ctx, w, std::max<size_t>(A1 * 4, want(n_al, 4)) + 64, A0 * 4))) return rc;
-    for (int w : {B_SEQLEN, B_NCIG})
-        if ((rc = ensure_keep(ctx, w, std::max<size_t>(A1 * 2, want(n_al, 2)) + 64, A0 * 2))) return rc;
-    if ((rc = ensure_keep(ctx, B_FLAGS, std::max<size_t>(A1, want(n_al, 1)) + 64, A0))) return rc;
-    if ((rc = ensure_keep(ctx, B_CIGOPS, std::max<size_t>((T->ops_base + n_ops) * 4, want(n_ops, 4)) + 64, T->ops_base * 4))) return rc;
-    if ((rc = ensure_keep(ctx, B_SEQPOOL, std::max<size_t>((T->blk_base + n_blk) * blk_bytes, want(n_blk, blk_bytes)) + 256, T->blk_base * blk_bytes))) return rc;
+    const uint64_t have[3] = {A0, T->ops_base, T->blk_base}, add[3] = {n_al, n_ops, n_blk};
+    for (int k = 0; k < DS_N; ++k) {
+        const uint64_t h = have[DS_ARRAYS[k].count], a = add[DS_ARRAYS[k].count];
+        const size_t w = ds_width(k, T->seq_bits), pad = k == DS_SEQPOOL ? 256 : 64;
+        if ((rc = ensure_keep(ctx, B_CONTIG + k, std::max<size_t>((h + a) * w, want(a, w)) + pad, h * w))) return rc;
+    }
     // per-alignment scratch of this file: QNAME position / length, group heads, their running count
     size_t off2 = 0;
     auto carve2 = [&](size_t bytes) { size_t o = off2; off2 += (bytes + 255) & ~size_t(255); return o; };
@@ -497,10 +511,7 @@ static int tok_process(pp_ctx* ctx, TokState* T, const uint8_t* text, uint64_t n
 
     EmitArgs ea;
     ea.p = pa; ea.aln_base = A0; ea.ops_base = T->ops_base; ea.blk_base = T->blk_base;
-    ea.contig = ctx->b[B_CONTIG].as<uint32_t>(); ea.ref_start = ctx->b[B_REFSTART].as<uint32_t>(); ea.seq_off = ctx->b[B_SEQOFF].as<uint32_t>();
-    ea.cigar_off = ctx->b[B_CIGOFF].as<uint32_t>(); ea.nm = ctx->b[B_NM].as<uint32_t>(); ea.cigar_ops = ctx->b[B_CIGOPS].as<uint32_t>();
-    ea.seq_len = ctx->b[B_SEQLEN].as<uint16_t>(); ea.n_cigar = ctx->b[B_NCIG].as<uint16_t>();
-    ea.flags = ctx->b[B_FLAGS].as<uint8_t>(); ea.seq_pool = ctx->b[B_SEQPOOL].as<uint8_t>();
+    ea.d = ds_view(ctx->b + B_CONTIG);
     ea.name_pos = (unsigned long long*)(sc + o_np); ea.name_len = (uint32_t*)(sc + o_nl);
     const unsigned emit_grid = (unsigned)((n_lines + TK_LINE_THREADS - 1) / TK_LINE_THREADS);
     if (T->seq_bits == 4) k_tok_emit<4><<<emit_grid, TK_LINE_THREADS, 0, s>>>(ea);
@@ -515,8 +526,8 @@ static int tok_process(pp_ctx* ctx, TokState* T, const uint8_t* text, uint64_t n
         size_t tb = T->cub.cap;
         CK(cub::DeviceScan::InclusiveSum(T->cub.p, tb, head, rs, (int64_t)n_al, s));
     }
-    k_tok_groups<<<aln_grid, TK_LINE_THREADS, 0, s>>>(n_al, head, rs, T->read_base, T->careful ? 1 : 0, ctx->b[B_READID].as<uint32_t>() + A0,
-                                                       ea.seq_off + A0, ea.seq_len + A0, ea.flags + A0, T->d_st);
+    k_tok_groups<<<aln_grid, TK_LINE_THREADS, 0, s>>>(n_al, head, rs, T->read_base, T->careful ? 1 : 0, ea.d.read_id + A0,
+                                                       ea.d.seq_off + A0, ea.d.seq_len + A0, ea.d.flags + A0, T->d_st);
     uint32_t* h_reads = (uint32_t*)(T->h_tot + 3);
     CK(cudaMemcpyAsync(h_reads, rs + (n_al - 1), 4, cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(T->h_st, T->d_st, sizeof(TokStatus), cudaMemcpyDeviceToHost, s));
@@ -877,7 +888,46 @@ extern "C" int pp_tok_finish(pp_ctx* ctx) {
         CK(cudaGetLastError());
         std::vector<uint8_t>().swap(T->shard_bases);
     }
-    return pp_ctx_commit_dataset(ctx, T->aln_base, T->read_base, T->ops_base, T->blk_base * (T->seq_bits == 4 ? 16 : 32), (uint32_t)T->seq_bits);
+    return pp_ctx_commit_dataset(ctx, T->aln_base, T->read_base, T->ops_base, T->blk_base * ds_block_bytes(T->seq_bits), (uint32_t)T->seq_bits);
+}
+
+// fn(side, g) on every context S[g].ctx, each on its own host thread but the first, which runs on the calling thread; the first error
+// (its message moved to S[0]'s context) before PP_TOK_HOST, before PP_TOK_NEED8.
+template <class Side, class F>
+static int fx_all(std::vector<Side>& S, F&& fn) {
+    std::vector<int> rc(S.size(), PP_OK);
+    auto run = [&](size_t g) {
+        pp_ctx* ctx = S[g].ctx;
+        const cudaError_t e = cudaSetDevice(ctx->device);
+        rc[g] = e != cudaSuccess ? ctx->fail_cuda(e, "cudaSetDevice", __FILE__, __LINE__) : fn(S[g], (int)g);
+    };
+    std::vector<std::thread> th;
+    for (size_t g = 1; g < S.size(); ++g) th.emplace_back(run, g);
+    run(0);
+    for (auto& t : th) t.join();
+    for (size_t g = 0; g < S.size(); ++g)
+        if (rc[g] < 0) { if (g) S[0].ctx->err = S[g].ctx->err; return rc[g]; }
+    for (int want : {PP_TOK_HOST, PP_TOK_NEED8})
+        if (std::count(rc.begin(), rc.end(), want)) return want;
+    return PP_OK;
+}
+
+// A device-to-device copy on ctx's stream into dctx's memory: a peer copy between two devices.
+static int fx_copy(pp_ctx* ctx, pp_ctx* dctx, void* dst, const void* src, size_t bytes) {
+    if (!bytes) return PP_OK;
+    if (dctx->device == ctx->device) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    else CK(cudaMemcpyPeerAsync(dst, dctx->device, src, ctx->device, bytes, ctx->stream));
+    return PP_OK;
+}
+
+// Peer access from ctx's device to the other devices of ctxs: NVLink between the GPUs where the box has it.
+static void enable_peers(pp_ctx* ctx, pp_ctx* const* ctxs, size_t n) {
+    for (size_t o = 0; o < n; ++o)
+        if (ctxs[o]->device != ctx->device) {
+            int can = 0;
+            if (cudaDeviceCanAccessPeer(&can, ctx->device, ctxs[o]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[o]->device, 0);
+            cudaGetLastError();                                                        // (already enabled is fine)
+        }
 }
 
 // =====================================================================================================================
@@ -891,22 +941,27 @@ extern "C" int pp_tok_finish(pp_ctx* ctx) {
 // the piece sizes.  Then pp_tok_set_shard / pp_tok_finish on every GPU: foreign records become ghosts, the shard is binned.
 // =====================================================================================================================
 #define X_MAX_FILES 64
+struct XCount {                      // kept records, their CIGAR ops, their own sequence blocks, the read groups they start
+    uint32_t rec, ops, blk, grp;
+    uint32_t of(DsCount c) const { return c == DS_RECS ? rec : c == DS_OPS ? ops : blk; }
+};
 struct XPlan {                       // per (source, destination): where the pieces of each file go
     uint32_t n_files;
     uint32_t mark_aln[X_MAX_FILES + 1];                                   // first local record of file f
-    uint32_t dst_aln[X_MAX_FILES], dst_ops[X_MAX_FILES], dst_blk[X_MAX_FILES], dst_grp[X_MAX_FILES];   // position in the destination's dataset
+    XCount dst[X_MAX_FILES];                                              // position in the destination's dataset
 };
 
 __global__ void k_x_touch(const uint32_t* __restrict__ contig, const uint32_t* __restrict__ read_id, uint64_t n, const uint32_t* __restrict__ owner,
-                          uint32_t n_total, uint32_t read0, uint32_t* __restrict__ touch) {
+                          uint32_t n_total, uint32_t* __restrict__ touch) {
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint32_t c = contig[i];
         const uint32_t o = (c == PP_CONTIG_UNKNOWN || c >= n_total) ? 0u : owner[c];      // unknown RNAMEs stay with shard 0 (shard.cpp)
-        atomicOr(&touch[read_id[i] - read0], 1u << o);
+        atomicOr(&touch[read_id[i]], 1u << o);
     }
 }
 
-// kept record -> (1, its ops, its own sequence blocks, 1 if it starts a group); element n is the scans' total slot
+// kept record -> (1, its ops, its own sequence blocks, 1 if it starts a group); element n is the scans' total slot.  `read0` is always 0
+// (read ids are local to the source): ptxas gives the kernel two more registers without the subtraction.
 __global__ void k_x_flags(const uint32_t* __restrict__ read_id, const uint16_t* __restrict__ n_cigar, const uint16_t* __restrict__ seq_len,
                           const uint8_t* __restrict__ flags, uint64_t n, uint32_t read0, const uint32_t* __restrict__ touch, uint32_t dest,
                           uint32_t* __restrict__ f_rec, uint32_t* __restrict__ f_ops, uint32_t* __restrict__ f_blk, uint32_t* __restrict__ f_grp) {
@@ -922,52 +977,40 @@ __global__ void k_x_flags(const uint32_t* __restrict__ read_id, const uint16_t* 
 }
 
 __global__ void k_x_marks(const uint32_t* __restrict__ s_rec, const uint32_t* __restrict__ s_ops, const uint32_t* __restrict__ s_blk,
-                          const uint32_t* __restrict__ s_grp, XPlan plan, uint32_t* __restrict__ out) {
+                          const uint32_t* __restrict__ s_grp, XPlan plan, XCount* __restrict__ out) {
     const uint32_t f = threadIdx.x;
     if (f <= plan.n_files) {
         const uint32_t i = plan.mark_aln[f];
-        out[4 * f + 0] = s_rec[i]; out[4 * f + 1] = s_ops[i]; out[4 * f + 2] = s_blk[i]; out[4 * f + 3] = s_grp[i];
+        out[f] = XCount{s_rec[i], s_ops[i], s_blk[i], s_grp[i]};
     }
 }
 
-struct XArrays {
-    const uint32_t *contig, *ref_start, *read_id, *seq_off, *cigar_off, *nm, *cigar_ops;
-    const uint16_t *seq_len, *n_cigar;
-    const uint8_t *flags, *seq_pool;
-};
-struct XStage {
-    uint32_t *contig, *ref_start, *read_id, *seq_off, *cigar_off, *nm, *cigar_ops;
-    uint16_t *seq_len, *n_cigar;
-    uint8_t *flags, *seq_pool;
-};
-
 // records that own their sequence: where its first block goes (indexed by the OLD block offset, local to this source)
-__global__ void k_x_blockmap(XArrays a, uint64_t n, uint32_t blk0, const uint32_t* __restrict__ s_rec_flag, const uint32_t* __restrict__ s_rec,
-                             const uint32_t* __restrict__ s_blk, uint32_t* __restrict__ blockmap) {
+__global__ void k_x_blockmap(DsArrays a, uint64_t n, const uint32_t* __restrict__ s_rec, const uint32_t* __restrict__ s_blk, uint32_t* __restrict__ blockmap) {
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         if (s_rec[i + 1] == s_rec[i]) continue;                                        // not kept
         if (a.flags[i] & (PP_FLAG_SEQSTAR | PP_FLAG_NOSEQ)) continue;
-        blockmap[a.seq_off[i] - blk0] = s_blk[i];
+        blockmap[a.seq_off[i]] = s_blk[i];
     }
 }
 
-__global__ void k_x_pack(XArrays a, XStage st, uint64_t n, uint32_t blk0, uint32_t blk_bytes, XPlan plan, const uint32_t* __restrict__ s_rec,
-                         const uint32_t* __restrict__ s_ops, const uint32_t* __restrict__ s_blk, const uint32_t* __restrict__ s_grp,
-                         const uint32_t* __restrict__ blockmap, const uint32_t* __restrict__ marks /* scans at the file starts */) {
+__global__ void k_x_pack(DsArrays a, DsArrays st, uint64_t n, XPlan plan, const uint32_t* __restrict__ s_rec, const uint32_t* __restrict__ s_ops,
+                         const uint32_t* __restrict__ s_blk, const uint32_t* __restrict__ s_grp, const uint32_t* __restrict__ blockmap,
+                         const XCount* __restrict__ marks /* scans at the file starts */) {
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint32_t j = s_rec[i];
         if (s_rec[i + 1] == j) continue;                                               // not kept
         uint32_t f = 0;
         while (f + 1 < plan.n_files && i >= plan.mark_aln[f + 1]) ++f;
-        const uint32_t m_ops = marks[4 * f + 1], m_blk = marks[4 * f + 2], m_grp = marks[4 * f + 3];
+        const uint32_t m_ops = marks[f].ops, m_blk = marks[f].blk, m_grp = marks[f].grp;
         const uint8_t fl = a.flags[i];
         const bool starts = (i == 0 || a.read_id[i] != a.read_id[i - 1]);
         st.contig[j] = a.contig[i]; st.ref_start[j] = a.ref_start[i]; st.nm[j] = a.nm[i];
         st.seq_len[j] = a.seq_len[i]; st.n_cigar[j] = a.n_cigar[i]; st.flags[j] = fl;
-        st.read_id[j] = plan.dst_grp[f] + (s_grp[i] + (starts ? 1u : 0u) - 1u - m_grp);
-        st.cigar_off[j] = plan.dst_ops[f] + (s_ops[i] - m_ops);
+        st.read_id[j] = plan.dst[f].grp + (s_grp[i] + (starts ? 1u : 0u) - 1u - m_grp);
+        st.cigar_off[j] = plan.dst[f].ops + (s_ops[i] - m_ops);
         uint32_t so = 0;
-        if (!(fl & PP_FLAG_NOSEQ)) so = plan.dst_blk[f] + (blockmap[a.seq_off[i] - blk0] - m_blk);
+        if (!(fl & PP_FLAG_NOSEQ)) so = plan.dst[f].blk + (blockmap[a.seq_off[i]] - m_blk);
         st.seq_off[j] = so;
         const uint32_t nc = a.n_cigar[i], co = a.cigar_off[i];
         for (uint32_t t = 0; t < nc; ++t) st.cigar_ops[s_ops[i] + t] = a.cigar_ops[co + t];
@@ -975,7 +1018,7 @@ __global__ void k_x_pack(XArrays a, XStage st, uint64_t n, uint32_t blk0, uint32
 }
 
 // the sequence blocks of kept owners, 16 bytes per thread
-__global__ void k_x_pack_seq(XArrays a, XStage st, uint64_t n, uint32_t blk_bytes, const uint32_t* __restrict__ s_rec, const uint32_t* __restrict__ s_blk) {
+__global__ void k_x_pack_seq(DsArrays a, DsArrays st, uint64_t n, uint32_t blk_bytes, const uint32_t* __restrict__ s_rec, const uint32_t* __restrict__ s_blk) {
     const uint32_t per = blk_bytes / 16;
     for (uint64_t i = blockIdx.x * (uint64_t)(blockDim.x / 8) + threadIdx.x / 8; i < n; i += (uint64_t)gridDim.x * (blockDim.x / 8)) {
         if (s_rec[i + 1] == s_rec[i]) continue;
@@ -987,13 +1030,13 @@ __global__ void k_x_pack_seq(XArrays a, XStage st, uint64_t n, uint32_t blk_byte
     }
 }
 
-struct TokState::XState {            // one context's tokenised ranges, moved out of the dataset buffers
-    DevBuf b[11];                    // B_CONTIG .. B_SEQPOOL, in the enum's order
-    DevBuf stage[11], touch, fl[4], sc[4], blockmap, marks, cubtmp;
+struct TokState::XState {            // one context's tokenised ranges, moved out of the dataset buffers (same layout), as a source
+    DevBuf b[DS_N];
+    DevBuf stage[DS_N], touch, fl[4], sc[4], blockmap, marks, cubtmp;
     uint64_t n = 0, ops = 0, blk = 0, reads = 0;
     std::vector<TokState::Mark> mk;
     DevBuf d_owner;
-    uint32_t* h_marks = nullptr;     // pinned
+    XCount* h_marks = nullptr;       // pinned
     void release() { for (auto& x : b) x.release(); for (auto& x : stage) x.release(); touch.release(); for (auto& x : fl) x.release();
                      for (auto& x : sc) x.release(); blockmap.release(); marks.release(); cubtmp.release(); d_owner.release();
                      if (h_marks) cudaFreeHost(h_marks); h_marks = nullptr; }
@@ -1001,180 +1044,192 @@ struct TokState::XState {            // one context's tokenised ranges, moved ou
 static void free_xstate(TokState* T) { if (T->xs) { T->xs->release(); delete T->xs; T->xs = nullptr; } }
 namespace {
 typedef TokState::XState XSource;
-const int X_BUFS[11] = {B_CONTIG, B_REFSTART, B_READID, B_SEQOFF, B_SEQLEN, B_CIGOFF, B_NCIG, B_NM, B_FLAGS, B_CIGOPS, B_SEQPOOL};
+
+struct XSide {                       // one context of pp_tok_exchange_finish
+    pp_ctx* ctx = nullptr;
+    XSource* x = nullptr;
+    std::vector<XCount> cnt;         // [destination * n_files + file]: what this source sends
+    std::vector<XPlan> plan;         // [destination]
+};
+
+unsigned x_grid(const XSide& X) { return (unsigned)std::min<uint64_t>((X.x->n + 256) / 256 + 1, (uint64_t)X.ctx->sm_count * 32); }
+}  // namespace
+
+// The tokenised ranges of every context leave its dataset buffers (those receive the shard).  PP_TOK_HOST past the file limit.
+static int x_take(std::vector<XSide>& S, pp_ctx* const* ctxs, int seq_bits, size_t* n_files, uint64_t* total_aln) {
+    for (size_t g = 0; g < S.size(); ++g) {
+        pp_ctx* ctx = ctxs[g];
+        TokState* T = ctx->tok;
+        if (!T || !T->active || T->marks.size() < 2 || T->seq_bits != seq_bits) return ctxs[0]->fail(PP_ERR_ARG, "pp_tok_exchange_finish: a context without tokenised ranges");
+        if (g == 0) *n_files = T->marks.size() - 1;
+        if (T->marks.size() - 1 != *n_files || *n_files > X_MAX_FILES) return PP_TOK_HOST;
+        if (!T->xs) T->xs = new XSource();
+        XSource& x = *T->xs;
+        x.n = T->aln_base; x.ops = T->ops_base; x.blk = T->blk_base; x.reads = T->read_base; x.mk = T->marks;
+        for (int k = 0; k < DS_N; ++k) std::swap(x.b[k], ctx->b[B_CONTIG + k]);
+        *total_aln += x.n;
+        XPlan P;
+        memset(&P, 0, sizeof P);
+        P.n_files = (uint32_t)*n_files;
+        for (size_t f = 0; f <= *n_files; ++f) P.mark_aln[f] = (uint32_t)x.mk[f].aln;
+        S[g].ctx = ctx; S[g].x = &x; S[g].plan.assign(S.size(), P);
+    }
+    return PP_OK;
 }
 
-#define XCK(ctx_, x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { rc = (ctx_)->fail_cuda(e_, #x, __FILE__, __LINE__); goto done; } } while (0)
+// Source X's records bound for destination o: their flags (k_x_flags), the four exclusive scans over them, and the scans at the file
+// starts (k_x_marks, into X's marks).  Both passes run it.
+static int x_scan(XSide& X, int o) {
+    pp_ctx* ctx = X.ctx;
+    XSource& x = *X.x;
+    cudaStream_t st = ctx->stream;
+    const DsArrays A = ds_view(x.b);
+    uint32_t* fl[4] = {x.fl[0].as<uint32_t>(), x.fl[1].as<uint32_t>(), x.fl[2].as<uint32_t>(), x.fl[3].as<uint32_t>()};
+    uint32_t* sc[4] = {x.sc[0].as<uint32_t>(), x.sc[1].as<uint32_t>(), x.sc[2].as<uint32_t>(), x.sc[3].as<uint32_t>()};
+    k_x_flags<<<x_grid(X), 256, 0, st>>>(A.read_id, A.n_cigar, A.seq_len, A.flags, x.n, 0u, x.touch.as<uint32_t>(), (uint32_t)o, fl[0], fl[1], fl[2], fl[3]);
+    for (int k = 0; k < 4; ++k) {
+        size_t tb = x.cubtmp.cap;
+        CK(cub::DeviceScan::ExclusiveSum(x.cubtmp.p, tb, fl[k], sc[k], (int64_t)(x.n + 1), st));
+    }
+    k_x_marks<<<1, X_MAX_FILES + 1, 0, st>>>(sc[0], sc[1], sc[2], sc[3], X.plan[(size_t)o], x.marks.as<XCount>());
+    return PP_OK;
+}
+
+// Pass one, on source X (context g): the destinations of every read group (k_x_touch), then what each destination gets out of each file.
+static int x_count(XSide& X, int g, const uint32_t* owner, uint32_t n_total, size_t n_files) {
+    pp_ctx* ctx = X.ctx;
+    XSource& x = *X.x;
+    cudaStream_t st = ctx->stream;
+    const uint64_t n = x.n;
+    const int n_ctx = (int)X.plan.size();
+    CK(x.d_owner.ensure((size_t)n_total * 4 + 16));
+    CK(cudaMemcpyAsync(x.d_owner.p, owner, (size_t)n_total * 4, cudaMemcpyHostToDevice, st));
+    CK(x.touch.ensure((size_t)x.reads * 4 + 16));
+    CK(cudaMemsetAsync(x.touch.p, 0, (size_t)x.reads * 4 + 16, st));
+    for (int k = 0; k < 4; ++k) { CK(x.fl[k].ensure((n + 2) * 4)); CK(x.sc[k].ensure((n + 2) * 4)); }
+    CK(x.marks.ensure((X_MAX_FILES + 1) * sizeof(XCount)));
+    size_t tb = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int64_t)(n + 1), st));
+    CK(x.cubtmp.ensure(tb + 256));
+    const DsArrays A = ds_view(x.b);
+    if (n) k_x_touch<<<x_grid(X), 256, 0, st>>>(A.contig, A.read_id, n, x.d_owner.as<uint32_t>(), n_total, x.touch.as<uint32_t>());
+    X.cnt.assign((size_t)n_ctx * n_files, XCount{});
+    for (int oo = 0; oo < n_ctx; ++oo) {
+        const int o = (g + oo) % n_ctx;                                                // (the sources start on different destinations)
+        const int rc = x_scan(X, o);
+        if (rc != PP_OK) return rc;
+        CK(cudaMemcpyAsync(x.h_marks, x.marks.p, (n_files + 1) * sizeof(XCount), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        for (size_t f = 0; f < n_files; ++f) {
+            const XCount &a = x.h_marks[f], &b = x.h_marks[f + 1];
+            X.cnt[(size_t)o * n_files + f] = XCount{b.rec - a.rec, b.ops - a.ops, b.blk - a.blk, b.grp - a.grp};
+        }
+    }
+    return PP_OK;
+}
+
+// On the host: at destination o, file by file, the pieces of the sources in order - global SAM order is (file, range, line), which is
+// what the ordered depth needs.  Every destination's dataset buffers are sized for what it receives.  PP_TOK_HOST past the size limits.
+static int x_plan(std::vector<XSide>& S, size_t n_files, int seq_bits) {
+    for (size_t o = 0; o < S.size(); ++o) {
+        uint64_t rec = 0, ops = 0, blk = 0, grp = 0;
+        for (size_t f = 0; f < n_files; ++f)
+            for (XSide& X : S) {
+                X.plan[o].dst[f] = XCount{(uint32_t)rec, (uint32_t)ops, (uint32_t)blk, (uint32_t)grp};
+                const XCount& c = X.cnt[o * n_files + f];
+                rec += c.rec; ops += c.ops; blk += c.blk; grp += c.grp;
+            }
+        if (rec >= 0x7FFFFFFFull - 4096 || ops > 0xFFFFFFFFull || blk > 0xFFFFFFFFull || grp >= 0xFFFFFFFFull) return PP_TOK_HOST;
+        pp_ctx* ctx = S[o].ctx;
+        CK(cudaSetDevice(ctx->device));
+        const uint64_t cnt[3] = {rec, ops, blk};
+        for (int k = 0; k < DS_N; ++k) CK(ctx->b[B_CONTIG + k].ensure(ds_bytes(k, cnt, seq_bits) + 256));
+        TokState* T = ctx->tok;
+        T->aln_base = rec; T->ops_base = ops; T->blk_base = blk; T->read_base = grp;
+    }
+    return PP_OK;
+}
+
+// Pass two, on source X (context g): per destination the kept records compacted into the staging arrays with every offset renumbered
+// for its place there (k_x_blockmap, k_x_pack, k_x_pack_seq), then each file's piece - one contiguous run of the staging arrays -
+// copied into the destination's dataset.
+static int x_send(XSide& X, int g, const std::vector<XSide>& S, size_t n_files, int seq_bits) {
+    pp_ctx* ctx = X.ctx;
+    XSource& x = *X.x;
+    cudaStream_t st = ctx->stream;
+    const uint64_t n = x.n;
+    const uint64_t cnt[3] = {n, x.ops, x.blk};
+    for (int k = 0; k < DS_N; ++k) CK(x.stage[k].ensure(ds_bytes(k, cnt, seq_bits) + 256));
+    CK(x.blockmap.ensure((size_t)x.blk * 4 + 16));
+    const DsArrays A = ds_view(x.b), Z = ds_view(x.stage);
+    const uint32_t* sc[4] = {x.sc[0].as<uint32_t>(), x.sc[1].as<uint32_t>(), x.sc[2].as<uint32_t>(), x.sc[3].as<uint32_t>()};
+    const int n_ctx = (int)S.size();
+    for (int oo = 0; oo < n_ctx; ++oo) {
+        const int o = (g + oo) % n_ctx;
+        int rc = x_scan(X, o);
+        if (rc != PP_OK) return rc;
+        const XPlan& P = X.plan[(size_t)o];
+        if (n) {
+            k_x_blockmap<<<x_grid(X), 256, 0, st>>>(A, n, sc[0], sc[2], x.blockmap.as<uint32_t>());
+            k_x_pack<<<x_grid(X), 256, 0, st>>>(A, Z, n, P, sc[0], sc[1], sc[2], sc[3], x.blockmap.as<uint32_t>(), x.marks.as<XCount>());
+            k_x_pack_seq<<<(unsigned)std::min<uint64_t>((n + 31) / 32 + 1, (uint64_t)ctx->sm_count * 64), 256, 0, st>>>(A, Z, n, ds_block_bytes(seq_bits),
+                                                                                                               sc[0], sc[2]);
+        }
+        CK(cudaMemcpyAsync(x.h_marks, x.marks.p, (n_files + 1) * sizeof(XCount), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        pp_ctx* dctx = S[(size_t)o].ctx;
+        for (size_t f = 0; f < n_files; ++f)
+            for (int k = 0; k < DS_N; ++k) {
+                const DsCount c = DS_ARRAYS[k].count;
+                const size_t w = ds_width(k, seq_bits);
+                const uint64_t from = x.h_marks[f].of(c), to = P.dst[f].of(c);
+                rc = fx_copy(ctx, dctx, dctx->b[B_CONTIG + k].as<uint8_t>() + to * w, x.stage[k].as<uint8_t>() + from * w, (x.h_marks[f + 1].of(c) - from) * w);
+                if (rc != PP_OK) return rc;
+            }
+        CK(cudaStreamSynchronize(st));                                                 // (the staging arrays are reused for the next destination)
+    }
+    return PP_OK;
+}
+
+static int x_exchange(pp_ctx* const* ctxs, int n_ctx, const uint32_t* owner, uint32_t n_total, const uint32_t* const* local_of,
+                      const pp_contigs* shard_contigs, uint64_t* n_aln_total) {
+    std::vector<XSide> S((size_t)n_ctx);
+    const int seq_bits = ctxs[0]->tok ? ctxs[0]->tok->seq_bits : 4;
+    size_t n_files = 0;
+    uint64_t total_aln = 0;
+    int rc = x_take(S, ctxs, seq_bits, &n_files, &total_aln);
+    if (rc != PP_OK) return rc;
+    for (XSide& X : S) {
+        pp_ctx* ctx = X.ctx;
+        CK(cudaSetDevice(ctx->device));
+        if (!X.x->h_marks) CK(cudaHostAlloc((void**)&X.x->h_marks, (X_MAX_FILES + 1) * sizeof(XCount), cudaHostAllocDefault));
+        enable_peers(ctx, ctxs, (size_t)n_ctx);
+    }
+    // every source works through its destinations on its own stream, driven by its own host thread
+    if ((rc = fx_all(S, [&](XSide& X, int g) { return x_count(X, g, owner, n_total, n_files); })) != PP_OK) return rc;
+    if ((rc = x_plan(S, n_files, seq_bits)) != PP_OK) return rc;
+    if ((rc = fx_all(S, [&](XSide& X, int g) { return x_send(X, g, S, n_files, seq_bits); })) != PP_OK) return rc;
+    if (n_aln_total) *n_aln_total = total_aln;
+    // every GPU holds its groups in global SAM order: ghosts, the shard's contigs, binning
+    for (int o = 0; o < n_ctx; ++o) {
+        pp_ctx* ctx = ctxs[o];
+        if (cudaSetDevice(ctx->device) != cudaSuccess) return PP_ERR_CUDA;
+        rc = pp_tok_set_shard(ctx, local_of[o], n_total, &shard_contigs[o], o == 0);
+        if (rc == PP_OK) rc = pp_tok_finish(ctx);
+        if (rc != PP_OK) { if (ctx != ctxs[0]) ctxs[0]->err = ctx->err; return rc; }
+    }
+    return PP_OK;
+}
 
 extern "C" int pp_tok_exchange_finish(pp_ctx* const* ctxs, int n_ctx, const uint32_t* owner, uint32_t n_total, const uint32_t* const* local_of,
                                       const pp_contigs* shard_contigs, uint64_t* n_aln_total) {
     if (!ctxs || n_ctx < 1 || !owner || !local_of || !shard_contigs) return PP_ERR_ARG;
     if (n_ctx > 32) return PP_TOK_HOST;                                                // (one bit per destination in a group's mask: the host sharder takes over)
-    pp_ctx* c0 = ctxs[0];
-    int rc = PP_OK;
-    std::vector<XSource*> src((size_t)n_ctx, nullptr);
-    const int seq_bits = c0->tok ? c0->tok->seq_bits : 4;
-    const uint32_t blk_bytes = seq_bits == 4 ? 16 : 32;
-    size_t n_files = 0;
-    // counts[g][o][f][4]: what source g sends destination o out of file f
-    std::vector<uint32_t> counts;
-    uint64_t total_aln = 0;
-    // ---- the tokenised arrays leave the dataset buffers (those will receive the shard)
-    for (int g = 0; g < n_ctx; ++g) {
-        pp_ctx* ctx = ctxs[g];
-        TokState* T = ctx->tok;
-        if (!T || !T->active || T->marks.size() < 2 || T->seq_bits != seq_bits) { rc = c0->fail(PP_ERR_ARG, "pp_tok_exchange_finish: a context without tokenised ranges"); goto done; }
-        if (g == 0) n_files = T->marks.size() - 1;
-        if (T->marks.size() - 1 != n_files || n_files > X_MAX_FILES) { rc = PP_TOK_HOST; goto done; }
-        if (!T->xs) T->xs = new XSource();
-        src[g] = T->xs;
-        XSource& S = *src[g];
-        S.n = T->aln_base; S.ops = T->ops_base; S.blk = T->blk_base; S.reads = T->read_base; S.mk = T->marks;
-        for (int k = 0; k < 11; ++k) std::swap(S.b[k], ctx->b[X_BUFS[k]]);
-        total_aln += S.n;
-    }
-    counts.assign((size_t)n_ctx * n_ctx * n_files * 4, 0);
-    for (int g = 0; g < n_ctx; ++g) {
-        XCK(ctxs[g], cudaSetDevice(ctxs[g]->device));
-        if (!src[g]->h_marks) XCK(ctxs[g], cudaHostAlloc((void**)&src[g]->h_marks, (X_MAX_FILES + 1) * 4 * sizeof(uint32_t), cudaHostAllocDefault));
-        for (int o = 0; o < n_ctx; ++o)                                                // NVLink between the GPUs where the box has it
-            if (ctxs[o]->device != ctxs[g]->device) {
-                int can = 0;
-                if (cudaDeviceCanAccessPeer(&can, ctxs[g]->device, ctxs[o]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[o]->device, 0);
-                cudaGetLastError();                                                    // (already enabled is fine)
-            }
-    }
-
-    for (int pass = 0; pass < 2; ++pass) {
-        // pass 0: sizes of every piece; (host: where every piece goes, destination arrays); pass 1: pack and send
-        std::vector<std::vector<XPlan>> plans;
-        if (pass == 1) {
-            plans.assign((size_t)n_ctx, std::vector<XPlan>((size_t)n_ctx));
-            for (int o = 0; o < n_ctx; ++o) {
-                uint64_t at[4] = {0, 0, 0, 0};
-                for (size_t f = 0; f < n_files; ++f)
-                    for (int g = 0; g < n_ctx; ++g) {
-                        XPlan& P = plans[g][o];
-                        P.dst_aln[f] = (uint32_t)at[0]; P.dst_ops[f] = (uint32_t)at[1]; P.dst_blk[f] = (uint32_t)at[2]; P.dst_grp[f] = (uint32_t)at[3];
-                        const uint32_t* c = &counts[(((size_t)g * n_ctx + o) * n_files + f) * 4];
-                        for (int k = 0; k < 4; ++k) at[k] += c[k];
-                    }
-                if (at[0] >= 0x7FFFFFFFull - 4096 || at[1] > 0xFFFFFFFFull || at[2] > 0xFFFFFFFFull || at[3] >= 0xFFFFFFFFull) { rc = PP_TOK_HOST; goto done; }
-                pp_ctx* ctx = ctxs[o];
-                XCK(ctx, cudaSetDevice(ctx->device));
-                const size_t each[11] = {4, 4, 4, 4, 2, 4, 2, 4, 1, 4, blk_bytes};
-                const uint64_t cnt[11] = {at[0], at[0], at[0], at[0], at[0], at[0], at[0], at[0], at[0], at[1], at[2]};
-                for (int k = 0; k < 11; ++k) XCK(ctx, ctx->b[X_BUFS[k]].ensure((size_t)cnt[k] * each[k] + 256));
-                TokState* T = ctx->tok;
-                T->aln_base = at[0]; T->ops_base = at[1]; T->blk_base = at[2]; T->read_base = at[3];
-            }
-        }
-        // every source GPU works through its destinations on its own stream, driven by its own host thread
-        auto per_source = [&](int g) -> int {
-            pp_ctx* ctx = ctxs[g];
-            XSource& S = *src[g];
-            cudaStream_t st = ctx->stream;
-            uint32_t* hm = S.h_marks;
-            CK(cudaSetDevice(ctx->device));
-            const uint64_t n = S.n;
-            const uint32_t read0 = 0, blk0 = 0;
-            const unsigned grid = (unsigned)std::min<uint64_t>((n + 256) / 256 + 1, (uint64_t)ctx->sm_count * 32);
-            XArrays A{S.b[0].as<uint32_t>(), S.b[1].as<uint32_t>(), S.b[2].as<uint32_t>(), S.b[3].as<uint32_t>(), S.b[5].as<uint32_t>(), S.b[7].as<uint32_t>(),
-                      S.b[9].as<uint32_t>(), S.b[4].as<uint16_t>(), S.b[6].as<uint16_t>(), S.b[8].as<uint8_t>(), S.b[10].as<uint8_t>()};
-            const size_t each[11] = {4, 4, 4, 4, 2, 4, 2, 4, 1, 4, blk_bytes};
-            if (pass == 0) {
-                CK(S.d_owner.ensure((size_t)n_total * 4 + 16));
-                CK(cudaMemcpyAsync(S.d_owner.p, owner, (size_t)n_total * 4, cudaMemcpyHostToDevice, st));
-                CK(S.touch.ensure((size_t)S.reads * 4 + 16));
-                CK(cudaMemsetAsync(S.touch.p, 0, (size_t)S.reads * 4 + 16, st));
-                for (int k = 0; k < 4; ++k) { CK(S.fl[k].ensure((n + 2) * 4)); CK(S.sc[k].ensure((n + 2) * 4)); }
-                CK(S.marks.ensure((X_MAX_FILES + 1) * 16));
-                size_t tb = 0;
-                CK(cub::DeviceScan::ExclusiveSum(nullptr, tb, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int64_t)(n + 1), st));
-                CK(S.cubtmp.ensure(tb + 256));
-                if (n) k_x_touch<<<grid, 256, 0, st>>>(A.contig, A.read_id, n, S.d_owner.as<uint32_t>(), n_total, read0, S.touch.as<uint32_t>());
-            } else {
-                const uint64_t cnt[11] = {n, n, n, n, n, n, n, n, n, S.ops, S.blk};
-                for (int k = 0; k < 11; ++k) CK(S.stage[k].ensure((size_t)cnt[k] * each[k] + 256));
-                CK(S.blockmap.ensure((size_t)S.blk * 4 + 16));
-            }
-            XPlan base;
-            memset(&base, 0, sizeof base);
-            base.n_files = (uint32_t)n_files;
-            for (size_t f = 0; f <= n_files; ++f) base.mark_aln[f] = (uint32_t)S.mk[f].aln;
-            for (int oo = 0; oo < n_ctx; ++oo) {
-                const int o = (g + oo) % n_ctx;                                        // (the sources start on different destinations)
-                uint32_t* fl[4] = {S.fl[0].as<uint32_t>(), S.fl[1].as<uint32_t>(), S.fl[2].as<uint32_t>(), S.fl[3].as<uint32_t>()};
-                uint32_t* sc[4] = {S.sc[0].as<uint32_t>(), S.sc[1].as<uint32_t>(), S.sc[2].as<uint32_t>(), S.sc[3].as<uint32_t>()};
-                k_x_flags<<<grid, 256, 0, st>>>(A.read_id, A.n_cigar, A.seq_len, A.flags, n, read0, S.touch.as<uint32_t>(), (uint32_t)o, fl[0], fl[1], fl[2], fl[3]);
-                for (int k = 0; k < 4; ++k) {
-                    size_t tb = S.cubtmp.cap;
-                    CK(cub::DeviceScan::ExclusiveSum(S.cubtmp.p, tb, fl[k], sc[k], (int64_t)(n + 1), st));
-                }
-                XPlan P = pass == 1 ? plans[g][o] : base;
-                P.n_files = base.n_files;
-                memcpy(P.mark_aln, base.mark_aln, sizeof base.mark_aln);
-                k_x_marks<<<1, X_MAX_FILES + 1, 0, st>>>(sc[0], sc[1], sc[2], sc[3], P, S.marks.as<uint32_t>());
-                if (pass == 1 && n) {
-                    XStage Z{S.stage[0].as<uint32_t>(), S.stage[1].as<uint32_t>(), S.stage[2].as<uint32_t>(), S.stage[3].as<uint32_t>(), S.stage[5].as<uint32_t>(),
-                             S.stage[7].as<uint32_t>(), S.stage[9].as<uint32_t>(), S.stage[4].as<uint16_t>(), S.stage[6].as<uint16_t>(), S.stage[8].as<uint8_t>(),
-                             S.stage[10].as<uint8_t>()};
-                    k_x_blockmap<<<grid, 256, 0, st>>>(A, n, blk0, fl[0], sc[0], sc[2], S.blockmap.as<uint32_t>());
-                    k_x_pack<<<grid, 256, 0, st>>>(A, Z, n, blk0, blk_bytes, P, sc[0], sc[1], sc[2], sc[3], S.blockmap.as<uint32_t>(), S.marks.as<uint32_t>());
-                    k_x_pack_seq<<<(unsigned)std::min<uint64_t>((n + 31) / 32 + 1, (uint64_t)ctx->sm_count * 64), 256, 0, st>>>(A, Z, n, blk_bytes, sc[0], sc[2]);
-                }
-                CK(cudaMemcpyAsync(hm, S.marks.p, (n_files + 1) * 16, cudaMemcpyDeviceToHost, st));
-                CK(cudaStreamSynchronize(st));
-                if (pass == 0) {
-                    for (size_t f = 0; f < n_files; ++f)
-                        for (int k = 0; k < 4; ++k)
-                            counts[(((size_t)g * n_ctx + o) * n_files + f) * 4 + k] = hm[4 * (f + 1) + k] - hm[4 * f + k];
-                    continue;
-                }
-                // the pieces travel: file f's kept records are one contiguous run of the staging arrays
-                pp_ctx* dctx = ctxs[o];
-                for (size_t f = 0; f < n_files; ++f) {
-                    const uint32_t* m0 = hm + 4 * f;
-                    const uint32_t* m1 = hm + 4 * (f + 1);
-                    for (int k = 0; k < 11; ++k) {
-                        const int q = k == 9 ? 1 : k == 10 ? 2 : 0;                   // which scan measures this array
-                        const uint64_t from = m0[q], cntk = (uint64_t)m1[q] - m0[q];
-                        const uint64_t to = q == 0 ? P.dst_aln[f] : q == 1 ? P.dst_ops[f] : P.dst_blk[f];
-                        if (!cntk) continue;
-                        uint8_t* dst = dctx->b[X_BUFS[k]].as<uint8_t>() + (size_t)to * each[k];
-                        const uint8_t* sp = S.stage[k].as<uint8_t>() + (size_t)from * each[k];
-                        if (dctx->device == ctx->device) CK(cudaMemcpyAsync(dst, sp, (size_t)cntk * each[k], cudaMemcpyDeviceToDevice, st));
-                        else CK(cudaMemcpyPeerAsync(dst, dctx->device, sp, ctx->device, (size_t)cntk * each[k], st));
-                    }
-                }
-                CK(cudaStreamSynchronize(st));                                         // (the staging arrays are reused for the next destination)
-            }
-            return PP_OK;
-        };
-        std::vector<int> prc((size_t)n_ctx, PP_OK);
-        {
-            std::vector<std::thread> th;
-            for (int g = 1; g < n_ctx; ++g) th.emplace_back([&, g] { prc[(size_t)g] = per_source(g); });
-            prc[0] = per_source(0);
-            for (auto& t : th) t.join();
-        }
+    const int rc = x_exchange(ctxs, n_ctx, owner, n_total, local_of, shard_contigs, n_aln_total);
+    // (the buffers stay with the context: the range arrays that were swapped out are the spare capacity of the next call)
+    if (rc != PP_OK)
         for (int g = 0; g < n_ctx; ++g)
-            if (prc[(size_t)g] != PP_OK) { rc = prc[(size_t)g]; if (ctxs[g] != c0) c0->err = ctxs[g]->err; goto done; }
-    }
-    // ---- every GPU holds its groups in global SAM order: ghosts, the shard's contigs, binning
-    for (int o = 0; o < n_ctx && rc == PP_OK; ++o) {
-        pp_ctx* ctx = ctxs[o];
-        if (cudaSetDevice(ctx->device) != cudaSuccess) { rc = PP_ERR_CUDA; break; }
-        rc = pp_tok_set_shard(ctx, local_of[o], n_total, &shard_contigs[o], o == 0);
-        if (rc == PP_OK) rc = pp_tok_finish(ctx);
-        if (rc != PP_OK && ctx != c0) c0->err = ctx->err;
-    }
-    if (n_aln_total) *n_aln_total = total_aln;
-done:
-    for (int g = 0; g < n_ctx; ++g) {
-        // (the buffers stay with the context: the range arrays that were swapped out are the spare capacity of the next call)
-        if (rc != PP_OK && ctxs[g]->tok) ctxs[g]->tok->active = false;
-    }
+            if (ctxs[g]->tok) ctxs[g]->tok->active = false;
     return rc;
 }
 
@@ -1195,15 +1250,13 @@ extern "C" int pp_dataset_download(pp_ctx* ctx, const pp_alignments* into) {
         return ctx->fail(PP_ERR_ARG, "pp_dataset_download: sizes differ from pp_dataset_sizes");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
-    const size_t n = (size_t)ctx->n_aln;
-    auto get = [&](const void* dst, int which, size_t bytes) -> cudaError_t {
-        if (!dst || !bytes) return cudaSuccess;
-        return cudaMemcpyAsync(const_cast<void*>(dst), ctx->b[which].p, bytes, cudaMemcpyDeviceToHost, s);
-    };
-    CK(get(into->contig, B_CONTIG, n * 4)); CK(get(into->ref_start, B_REFSTART, n * 4)); CK(get(into->read_id, B_READID, n * 4));
-    CK(get(into->seq_off, B_SEQOFF, n * 4)); CK(get(into->seq_len, B_SEQLEN, n * 2)); CK(get(into->cigar_off, B_CIGOFF, n * 4));
-    CK(get(into->n_cigar, B_NCIG, n * 2)); CK(get(into->nm, B_NM, n * 4)); CK(get(into->flags, B_FLAGS, n));
-    CK(get(into->cigar_ops, B_CIGOPS, (size_t)ctx->n_ops * 4)); CK(get(into->seq_pool, B_SEQPOOL, (size_t)ctx->seq_bytes));
+    const void* host[DS_N];
+    ds_host(into, host);
+    const uint64_t cnt[3] = {ctx->n_aln, ctx->n_ops, 0};
+    for (int k = 0; k < DS_N; ++k) {
+        const size_t bytes = k == DS_SEQPOOL ? (size_t)ctx->seq_bytes : ds_bytes(k, cnt, ctx->seq_bits);   // (an uploaded pool may end inside a block)
+        if (host[k] && bytes) CK(cudaMemcpyAsync(const_cast<void*>(host[k]), ctx->b[B_CONTIG + k].p, bytes, cudaMemcpyDeviceToHost, s));
+    }
     CK(cudaStreamSynchronize(s));
     return PP_OK;
 }
@@ -1448,24 +1501,11 @@ static int download_stream(int device, TokState* T, const uint8_t* src, int fd, 
 static int ftok_lines(pp_ctx* ctx, TokState* T, int which, const uint8_t* text, uint64_t n, bool unterminated, DevBuf& lines, DevBuf& tmp, FStatus* d_st,
                       FileDev* fd, uint32_t* launches) {
     cudaStream_t s = ctx->stream;
-    const uint64_t n16 = (n + 15) & ~15ull;
-    const uint64_t n_tiles = (n16 + TK_TILE - 1) / TK_TILE;
-    if (n_tiles == 0 || n_tiles >= 0x7FFFFFFFull) return PP_TOK_HOST;
-    size_t cub_bytes = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int64_t)(n_tiles + 1)));
-    CK(T->cub.ensure(cub_bytes + 256));
-    TRY_ALLOC(ctx->b[B_TOKLINE].ensure((n_tiles + 2) * 8));
-    unsigned long long* tile_cnt = ctx->b[B_TOKLINE].as<unsigned long long>();
-    CK(cudaMemsetAsync(tile_cnt + n_tiles, 0, 8, s));
-    k_tok_count<<<(unsigned)n_tiles, TK_THREADS, 0, s>>>(text, n16, tile_cnt);
-    {
-        size_t tb = T->cub.cap;
-        CK(cub::DeviceScan::ExclusiveSum(T->cub.p, tb, tile_cnt, tile_cnt, (int64_t)(n_tiles + 1), s));
-    }
-    CK(cudaMemcpyAsync(T->h_tot, tile_cnt + n_tiles, 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    const uint64_t n_lines = T->h_tot[0] + (unterminated ? 1 : 0);
-    if (n_lines == 0 || n_lines >= 0xFFFFFFF0ull) return PP_TOK_HOST;
+    LineIndex li;
+    const int rc = line_count(ctx, T, text, n, unterminated, &li);
+    if (rc != PP_OK) return rc;
+    const uint64_t n_lines = li.n_lines;
+    if (n_lines == 0) return PP_TOK_HOST;
     TRY_ALLOC(lines.ensure((n_lines + 2) * 8));
     size_t off = 0;
     auto carve = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~size_t(255); return o; };
@@ -1476,8 +1516,9 @@ static int ftok_lines(pp_ctx* ctx, TokState* T, int which, const uint8_t* text, 
     fd->line_start = lines.as<unsigned long long>();
     fd->recs = (tok::FLineRec*)(b + o_rec); fd->s_al = (unsigned long long*)(b + o_al);
     fd->name_slot = (uint32_t*)(b + o_ns); fd->ref_slot = (uint32_t*)(b + o_rs);
-    k_tok_index<<<(unsigned)n_tiles, TK_THREADS, 0, s>>>(text, n16, tile_cnt, lines.as<unsigned long long>());
+    line_starts(ctx, text, li, lines.as<unsigned long long>());
     k_ftok_parse<<<(unsigned)((n_lines + 1 + TK_LINE_THREADS - 1) / TK_LINE_THREADS), TK_LINE_THREADS, 0, s>>>(*fd, which, d_st);
+    size_t cub_bytes = 0;
     CK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, fd->s_al, fd->s_al, (int64_t)(n_lines + 1)));
     CK(T->cub.ensure(cub_bytes + 256));
     {
@@ -1681,34 +1722,6 @@ struct FilterSide {
 };
 
 }  // namespace
-
-// fn(side, g) on every context, each on its own host thread but the first, which runs on the calling thread; the first error (its
-// message moved to ctxs[0]) before PP_TOK_HOST, before PP_TOK_NEED8.
-template <class F>
-static int fx_all(std::vector<FilterSide>& S, F&& fn) {
-    std::vector<int> rc(S.size(), PP_OK);
-    auto run = [&](size_t g) {
-        pp_ctx* ctx = S[g].ctx;
-        const cudaError_t e = cudaSetDevice(ctx->device);
-        rc[g] = e != cudaSuccess ? ctx->fail_cuda(e, "cudaSetDevice", __FILE__, __LINE__) : fn(S[g], (int)g);
-    };
-    std::vector<std::thread> th;
-    for (size_t g = 1; g < S.size(); ++g) th.emplace_back(run, g);
-    run(0);
-    for (auto& t : th) t.join();
-    for (size_t g = 0; g < S.size(); ++g)
-        if (rc[g] < 0) { if (g) S[0].ctx->err = S[g].ctx->err; return rc[g]; }
-    for (int want : {PP_TOK_HOST, PP_TOK_NEED8})
-        if (std::count(rc.begin(), rc.end(), want)) return want;
-    return PP_OK;
-}
-
-static int fx_copy(pp_ctx* ctx, pp_ctx* dctx, void* dst, const void* src, size_t bytes) {
-    if (!bytes) return PP_OK;
-    if (dctx->device == ctx->device) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-    else CK(cudaMemcpyPeerAsync(dst, dctx->device, src, ctx->device, bytes, ctx->stream));
-    return PP_OK;
-}
 
 // Text in, on one context: both texts into HBM, the second streaming in while the first is indexed and parsed (ftok_lines; an empty
 // range is skipped), and the aligned counts.  With `cuts` the context reads bytes [cuts[f][g], cuts[f][g + 1]) of file f, else the
@@ -2171,12 +2184,7 @@ int pp_filter_files_device(pp_ctx* const* ctxs, int n_ctx, const char* in1, cons
         if (rc) { if (g) c0->err = ctx->err; return rc; }
         if (!S[g].T->fbufs) S[g].T->fbufs = new TokFilterBufs();
         S[g].B = S[g].T->fbufs;
-        for (uint32_t o = 0; o < n; ++o)                                    // NVLink between the GPUs where the box has it
-            if (ctxs[o]->device != ctx->device) {
-                int can = 0;
-                if (cudaDeviceCanAccessPeer(&can, ctx->device, ctxs[o]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[o]->device, 0);
-                cudaGetLastError();                                          // (already enabled is fine)
-            }
+        enable_peers(ctx, ctxs, n);
     }
 
     // ---- every context: its two texts into HBM, lines, quick parse
